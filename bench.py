@@ -1,11 +1,12 @@
 #!/usr/bin/env python3
 """bench.py — query+ctx pairs/sec of the bi-encoder contrastive training step (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path (one rank per GPU)
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path (one rank per GPU)
+  python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed (.npy)
   python bench.py --impl reference ...                      # the reference's own CPU path (HF + torch, fp32)
   python bench.py --impl stock ...                          # stock HF + PyTorch on the same GPU (the 1.5x denominator)
 
-The default (b200) line also carries: `stock_gpu` / `vs_stock` (stock HF + PyTorch on the SAME GPU right after our arm -
+The default line also carries: `stock_gpu` / `vs_stock` (stock HF + PyTorch on the SAME GPU right after our arm -
 the denominator of north_star's 1.5x target), `phases` (CUDA-event time per phase of the step), `selfcheck` (N > 1:
 NCCL parity against the reference-generated goldens before timing) and, at N > 1, `grad_allreduce_bf16` (the same step
 with the `fp16_grads` compressed gradient all-reduce).
@@ -40,22 +41,22 @@ WORKLOADS = {
     # name: (model cfg, queries/GPU, hard negs, seq len)
     "bert-base_s128_b128_n7": (BERT_BASE, 128, 7, 128),          # BASELINE configs[1] / [2]  (the headline)
     "bert-base_s64_b8_n1": (BERT_BASE, 8, 1, 64),                # configs[0] shape
-    "roberta-large_s256_b64_n15": (ROBERTA_LARGE, 64, 15, 256),  # configs[3] (needs activation chunking, see below)
+    "roberta-large_s256_b16_n15": (ROBERTA_LARGE, 16, 15, 256),  # configs[3]'s model and recipe at an 80 GB batch
 }
-# configs[3] (RoBERTa-large, 278 528 tokens x 24 layers per GPU) needs ~214 GB of saved activations in the full mode:
-# it runs with LEAN activations (22 KB instead of 32 KB per token and layer; gelu / gelu' / attention output rebuilt in
-# backward), which fits 180 GB without recomputing the forward.  --act-chunk N selects the older chunked-recompute path.
+# RoBERTa-large runs with LEAN activations (22 KB instead of 32 KB per token and layer; gelu / gelu' / attention output
+# rebuilt in backward): 69 632 tokens x 24 layers per GPU then fit an 80 GB H100 without recomputing the forward.
+# --act-chunk N selects the older chunked-recompute path.
 ACT_CHUNK = {}
-LEAN = {"roberta-large_s256_b64_n15"}
+LEAN = {"roberta-large_s256_b16_n15"}
 
 
 def flops_per_token_train(cfg, S):
     H, I, L = cfg["hidden_size"], cfg["intermediate_size"], cfg["num_hidden_layers"]
-    return 3 * L * (2 * (4 * H * H + 2 * H * I) + 4 * S * H)  # SURVEY.md §8d
+    return 3 * L * (2 * (4 * H * H + 2 * H * I) + 4 * S * H)  # fwd + bwd = 3 x fwd: QKV / out / FFN GEMMs + QK^T and PV
 
 
 def synth_batch(rank, cfg, B, n, S, pin=True):
-    """BASELINE.md §5 variant A: all sequences exactly S tokens, mask all ones."""
+    """Benchmark inputs, variant A: all sequences exactly S tokens, mask all ones."""
     g = torch.Generator().manual_seed(1234 + rank)
     C = B * (1 + n)
 
@@ -151,8 +152,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, sustained)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3)"
 
 
 # --------------------------------------------------------------------------------------- CPU reference path
@@ -377,7 +378,7 @@ def selfcheck(world, rank, dev):
 
 
 def dataloader_leg(trainer, dev, B, n, S, steps, warmup):
-    """SURVEY.md 8(d): 'plus one end-to-end number including the dataloader'.  A synthetic DPR-format JSONL (texts long
+    """One end-to-end number including the dataloader.  A synthetic DPR-format JSONL (texts long
     enough that every sequence truncates to exactly S tokens, i.e. the named shape) goes through the repo's input
     pipeline - mmap line index, JSON + negative sampling, tokenisation, pinned staging, side-stream H2D - while the GPU
     trains; the loss is read back every step.  Returns (ms per step, rows per batch)."""
@@ -436,7 +437,25 @@ def dataloader_leg(trainer, dev, B, n, S, steps, warmup):
         shutil.rmtree(tmp, ignore_errors=True)
 
 
-def run_b200(args, workload):
+DUMP_SAMPLE = 1 << 21   # parameters sampled per encoder (8 MB of float32 each)
+
+
+def dump_outputs(out_dir, loss, task):
+    """What the last timed training step left to its caller: the loss it returned and the parameters its optimizer step
+    wrote (both encoders; a fixed, seeded sample of each flat parameter vector, the same indices in every run).  The
+    pooler, which the CLS-pooled path never reads, is left out."""
+    import numpy as np
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss)], dtype=np.float64))
+    for name, enc in (("query_encoder", task.query_encoder), ("context_encoder", task.context_encoder)):
+        flat = torch.cat([p.detach().reshape(-1).float() for n, p in enc.named_parameters() if ".pooler." not in n])
+        g = torch.Generator().manual_seed(2024)
+        idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+        np.save(os.path.join(out_dir, f"{name}_params_sample.npy"), flat[idx.to(flat.device)].cpu().numpy())
+
+
+def run_dprb(args, workload):
     from dpr_scale_b200 import _lib, ops
     from dpr_scale_b200.task.dpr_task import DenseRetrieverTask, _ScoreCE
     from dpr_scale_b200.trainer import Trainer
@@ -467,6 +486,9 @@ def run_b200(args, workload):
     with contextlib.redirect_stdout(sys.stderr):      # stdout carries exactly ONE line: the JSON result
         trainer.attach(task, None, "fit")
     task.train()
+    # fixed dropout streams (the default base mixes in the module's address): with the same arguments every run draws
+    # the same masks, so two builds can be compared output for output
+    task.query_encoder._drop_base, task.context_encoder._drop_base = 0x5EED0001, 0x5EED0002
     task.context_encoder.activation_chunk = ACT_CHUNK.get(workload, 0) if args.act_chunk < 0 else args.act_chunk
     lean = (workload in LEAN and task.context_encoder.activation_chunk == 0) or args.lean
     task.context_encoder.lean_activations = task.query_encoder.lean_activations = lean
@@ -501,9 +523,19 @@ def run_b200(args, workload):
     if rank == 0:
         sampler.start()
     launches0 = ops.launch_count()
-    ms_step = timed(lambda i: trainer.training_step(dev_batch, i), args.steps)
+    last = {}
+
+    def kernel_step(i):
+        # detached: the returned loss holds the step's autograd graph, whose nodes reference both encoders and their
+        # activation workspaces; keeping it would keep all of that alive into the stock leg below
+        last["loss"] = trainer.training_step(dev_batch, i).detach()
+
+    ms_step = timed(kernel_step, args.steps)
     launches = ops.launch_count() - launches0        # counted inside the C launchers (dprb_launch_count)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], task)
+    del last
 
     # ---- roofline leg: the same step, timed again with CUDA events around EVERY GEMM launch.  The query encoder is
     # kept on the main stream here (no two-stream overlap), otherwise launch intervals of the two streams interleave
@@ -610,7 +642,7 @@ def run_b200(args, workload):
                    "global_batch": pairs_step, "parallelism": f"dp{world}", "negatives": "global in-batch" if world > 1 else "in-batch",
                    "optimizer": "fused AdamW + clip 2.0 + LambdaLR", "dropout": args.dropout,
                    "grad_allreduce": (args.grad_dtype + (" (reference default: fp16_grads=false)" if args.grad_dtype == "fp32" else " (fp16_grads=true)")) if world > 1 else None,
-                   "l2": "working set (>=40 GB activations + 0.9 GB weights/step) exceeds the 126 MB L2; no flush needed"},
+                   "l2": "working set (tens of GB of activations + 0.9 GB weights/step) exceeds the 50 MB L2; no flush needed"},
         "e2e": {"value": pairs_step / (ms_e2e / 1e3), "unit": "pairs/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": batch_bytes(host_batch), "d2h_bytes_per_step": 4,
                 "d2h": "every step's loss copied to pinned host memory in the step, read by the host one step later"},
@@ -619,15 +651,10 @@ def run_b200(args, workload):
         "gpu_launches_how": "dprb_launch_count(): incremented at every kernel launch inside libdprb.so, difference over the timed region",
         "clocks": clocks,
         "peak_mem_gb": peak_mem,
-        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel<*,*,2> (tcgen05 cta_group::2 UMMA 256x256x16)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel<*,*,*> (wgmma m64n128k16, 128x128 tiles)",
                      "achieved": gemm_tflops, "peak": peak_tf, "unit": "TFLOP/s", "frac": gemm_tflops / peak_tf,
                      "peak_source": peak_src,
-                     # not measured by this run: one `ncu --set full` capture of the largest launch of this kernel
-                     # (FFN-in, M=131072 N=3072 K=768), dram read+write vs its algorithmic bytes (A + 2 outputs + W)
                      "traffic": None,
-                     "traffic_ncu": ({"bytes": 1.766e9, "algorithmic_bytes": 1.816e9, "launch": "FFN-in M131072 N3072 K768",
-                                      "source": "profiles/r1_final_ncu_full_summary.json (ncu --set full, separate run)"}
-                                     if workload == "bert-base_s128_b128_n7" else None),
                      "gemm_launches": nl.value,
                      "gemm_ms_per_step": tms.value / prof_steps, "roofline_region_ms_per_step": ms_prof,
                      "gemm_share_of_step": (tms.value / prof_steps) / ms_prof,
@@ -664,7 +691,7 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference", "stock"])
+    ap.add_argument("--impl", default="dprb", choices=["dprb", "reference", "stock"])
     ap.add_argument("--workload", default="bert-base_s128_b128_n7", choices=sorted(WORKLOADS))
     ap.add_argument("--ref-pairs", type=int, default=1, help="pairs per step of the bounded CPU sample (--impl reference)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -678,12 +705,14 @@ def main():
                     help="gradient all-reduce precision at N > 1 (fp32 = the reference default fp16_grads=false)")
     ap.add_argument("--lean", action="store_true", help="lean activations (save_for_backward = 2) whatever the workload")
     ap.add_argument("--act-chunk", type=int, default=-1, help="override the activation chunk (sequences) of the context encoder")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args, args.workload)
     if args.impl == "stock":
         return run_stock(args, args.workload)
-    return run_b200(args, args.workload)
+    return run_dprb(args, args.workload)
 
 
 if __name__ == "__main__":

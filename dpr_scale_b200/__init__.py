@@ -1,4 +1,4 @@
-"""dpr_scale_b200 — B200-native (sm_100a) bi-encoder training path behind dpr-scale's plugin surface.
+"""dpr_scale_b200 — H100-native (sm_90a) bi-encoder training path behind dpr-scale's plugin surface.
 
 Only what the hot path needs lives here: ``csrc/`` (CUDA kernels + the C ABI of ``include/dprb.h``),
 ``_lib`` (ctypes binding), ``ops`` (tensor-level wrappers), ``models`` / ``task`` (mirrors of

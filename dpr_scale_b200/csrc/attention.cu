@@ -1,14 +1,8 @@
-// Self-attention core (head_dim 64, S <= 256) forward + backward: dispatch to the tcgen05 kernels.
+// Self-attention core (head_dim 64, S <= 256) forward + backward: shape checks, then the wgmma kernels of
+// attention_wgmma.cu (keys padded to 64, 128 or 256).
 //
-// Replaces BertSelfAttention.forward's scaled_dot_product_attention
-// (site-packages/transformers/models/bert/modeling_bert.py:168-207 and
-// integrations/sdpa_attention.py:92-101) and its autograd backward, as reached from
-// /root/reference/dpr_scale/models/hf_model.py:38.
-//
-//   S <= 128        attention_tc.cu     one (sequence, head) = one 128-row UMMA tile
-//   128 < S <= 256  attention_tc256.cu  two 128-row tiles per (sequence, head)
-// (The round-1 mma.sync kernels that used to live here as an A/B fallback are gone: nothing on the product path
-// compiles to HMMA any more - profiles/r2/sass_evidence.txt.)
+// Replaces BertSelfAttention.forward's scaled_dot_product_attention (transformers' modeling_bert.py) and its
+// autograd backward.
 //
 // Layout: qkv bf16 [nseq*S, 3H], row t = (seq, s); Q at column h*64, K at H + h*64, V at 2H + h*64.
 #include "common.cuh"
@@ -31,19 +25,17 @@ int attn_fwd_lse(const void* qkv, const int32_t* attn_mask, void* ctx, float* ls
                  float dropout_p, unsigned long long site_seed, cudaStream_t stream) {
   if (int rc = check_shape(nseq, S, heads, "attn_fwd")) return rc;
   if (nseq == 0) return 0;
-  if (S <= 128) return attn_fwd_tc(qkv, attn_mask, ctx, lse, nseq, S, heads, dropout_p, site_seed, stream);
-  return attn_fwd_tc2(qkv, attn_mask, ctx, lse, nseq, S, heads, dropout_p, site_seed, stream);  // 128 < S <= 256
+  return attn_fwd_wg(qkv, attn_mask, ctx, lse, nseq, S, heads, dropout_p, site_seed, stream);
 }
 
 int attn_bwd_lse(const void* qkv, const int32_t* attn_mask, const void* ctx, const float* lse, const void* dctx,
                  void* dqkv, float* dbias, int nseq, int S, int heads, float dropout_p,
                  unsigned long long site_seed, cudaStream_t stream) {
+  (void)ctx;   // D = rowsum(P * dP) is rebuilt in fp32 from Q, K, V, dO and lse
   if (int rc = check_shape(nseq, S, heads, "attn_bwd")) return rc;
   if (nseq == 0) return 0;
-  if (S <= 128)
-    return attn_bwd_tc(qkv, attn_mask, lse, dctx, dqkv, dbias, nseq, S, heads, dropout_p, site_seed, stream);
-  // 128 < S <= 256: the QKV bias gradient is a separate streaming pass
-  if (int rc = attn_bwd_tc2(qkv, attn_mask, ctx, lse, dctx, dqkv, nseq, S, heads, dropout_p, site_seed, stream)) return rc;
+  if (int rc = attn_bwd_wg(qkv, attn_mask, lse, dctx, dqkv, nseq, S, heads, dropout_p, site_seed, stream)) return rc;
+  // the QKV bias gradient: column sums of the bf16 dQ / dK / dV
   if (dbias != nullptr) return colsum_bf16(dqkv, 3LL * heads * DH, dbias, nseq * S, 3 * heads * DH, stream);
   return 0;
 }

@@ -1,12 +1,13 @@
-// dprb — B200 (sm_100a) kernels for the dpr-scale bi-encoder training path.
-// Shared device helpers: PTX wrappers for mbarrier / TMA / tcgen05 / TMEM, small math,
-// warp reductions, error plumbing.  Everything here is sm_100a-only by design.
+// dprb — H100 (sm_90a) kernels for the dpr-scale bi-encoder training path.
+// Shared device helpers: PTX wrappers for mbarrier / TMA / wgmma, small math,
+// warp reductions, error plumbing.  Everything here targets sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 #ifndef DPRB_HANG_GUARD
 #define DPRB_HANG_GUARD 1
@@ -86,6 +87,13 @@ __device__ __forceinline__ float2 unpack_f16x2(uint32_t u) {
 __device__ __forceinline__ uint32_t pack_16x2(float lo, float hi, bool f16) { return f16 ? pack_f16x2(lo, hi) : pack_bf16x2(lo, hi); }
 __device__ __forceinline__ float2 unpack_16x2(uint32_t u, bool f16) { return f16 ? unpack_f16x2(u) : unpack_bf16x2(u); }
 
+// Element pairs in fp32 with explicit rounding (no contraction), so every pair operation rounds exactly once.
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+
 // erf-GELU (HF "gelu", modeling_bert.py BertIntermediate) through a fitted Gaussian CDF:
 // Phi(x) = sigma(z(x)), z = a0 x + a1 x^3 + a2 x^5 (least-squares fit on [-6,6], argument clamped to [-8,8]):
 // max |Phi err| 5.8e-5, max |x*Phi - gelu_erf(x)| 3.0e-5 over all x, max |derivative err| 1.2e-4 — two orders of
@@ -118,29 +126,27 @@ __device__ __forceinline__ void gelu_and_grad(float x, float& g, float& gd) {
   g = x * sg;
   gd = sg * fmaf(xc * e * sg, inside, 1.f);
 }
-// The same function on PAIRS of elements with Blackwell's packed fp32 math (FFMA2 / FMUL2 / FADD2: one issue slot per
-// two elements).  At K = 768 the GEMM epilogue has ~24 issue slots per output element and the scalar form used ~20 of
-// them, which made the FFN-in GEMM epilogue-bound (632 us against 457 us with a plain bias epilogue).  Changes against
-// the scalar form, all exact in effect: the argument clamp becomes one min on x^2 (the fit's odd polynomial must not be
+// The same function on PAIRS of elements (the form every epilogue uses).  Changes against the scalar form, all exact
+// in effect: the argument clamp becomes one min on x^2 (the fit's odd polynomial must not be
 // evaluated beyond |x| = 8, where its x^5 term would turn it around); 1 - sigma replaces e * sigma (same quantity,
 // no inf * 0 when e overflows), which also removes the select that zeroed the derivative term in the clamped region.
 __device__ __forceinline__ void gelu_and_grad2(float2 x, float2& g, float2& gd) {
-  float2 x2 = __fmul2_rn(x, x);
+  float2 x2 = fmul2(x, x);
   x2.x = fminf(x2.x, 64.f);
   x2.y = fminf(x2.y, 64.f);
   const float2 one = make_float2(1.f, 1.f);
-  float2 pz = __ffma2_rn(x2, make_float2(1.03455483e-3f, 1.03455483e-3f), make_float2(-1.06900513e-1f, -1.06900513e-1f));
-  pz = __ffma2_rn(pz, x2, make_float2(-2.30098511f, -2.30098511f));
-  const float2 ex = __fmul2_rn(pz, x);
+  float2 pz = ffma2(x2, make_float2(1.03455483e-3f, 1.03455483e-3f), make_float2(-1.06900513e-1f, -1.06900513e-1f));
+  pz = ffma2(pz, x2, make_float2(-2.30098511f, -2.30098511f));
+  const float2 ex = fmul2(pz, x);
   const float2 e = make_float2(ex2_approx(ex.x), ex2_approx(ex.y));        // exp(-z)
-  const float2 den = __fadd2_rn(e, one);
+  const float2 den = fadd2(e, one);
   const float2 sg = make_float2(rcp_approx(den.x), rcp_approx(den.y));     // sigma(z) ~ Phi(x)
-  float2 zp = __ffma2_rn(x2, make_float2(-3.58549371e-3f, -3.58549371e-3f), make_float2(2.22293380e-1f, 2.22293380e-1f));
-  zp = __ffma2_rn(zp, x2, make_float2(1.59492135f, 1.59492135f));          // z'(x)
-  g = __fmul2_rn(x, sg);
-  const float2 t = __ffma2_rn(sg, make_float2(-1.f, -1.f), one);           // 1 - sigma
-  const float2 w = __ffma2_rn(__fmul2_rn(x, t), zp, one);
-  gd = __fmul2_rn(sg, w);
+  float2 zp = ffma2(x2, make_float2(-3.58549371e-3f, -3.58549371e-3f), make_float2(2.22293380e-1f, 2.22293380e-1f));
+  zp = ffma2(zp, x2, make_float2(1.59492135f, 1.59492135f));          // z'(x)
+  g = fmul2(x, sg);
+  const float2 t = ffma2(sg, make_float2(-1.f, -1.f), one);           // 1 - sigma
+  const float2 w = ffma2(fmul2(x, t), zp, one);
+  gd = fmul2(sg, w);
 }
 // Counter-based dropout RNG.  One 32-bit hash (lowbias32 finaliser, 9 integer instructions) decides TWO horizontally
 // adjacent elements (16 bits each), keyed by (row, column group of 8, pair in the group, site seed): element (r, c) is kept iff its 16-bit lane
@@ -281,84 +287,6 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 // all prior bulk stores of this thread have finished reading their shared-memory source
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread for the whole CTA.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <-> TMEM lane base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory matrix descriptor (SWIZZLE_128B, sm_100 "version 1").
-// Field layout follows the PTX ISA "tcgen05 matrix descriptor": start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version [46,48)=1, layout_type [61,64)=2 (128B swizzle).
-__device__ __forceinline__ uint64_t make_umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32, dense.
-// a_f16 / b_f16: that operand holds IEEE fp16 instead of bf16 (format code 0 instead of 1); the two may differ.
-__host__ __device__ constexpr uint32_t make_idesc_16_f32(int M, int N, int a_mn_major, int b_mn_major, int a_f16, int b_f16) {
-  return (1u << 4)                               // c_format = F32
-         | ((a_f16 ? 0u : 1u) << 7)              // a_format: 0 = F16, 1 = BF16
-         | ((b_f16 ? 0u : 1u) << 10)             // b_format
-         | ((uint32_t)a_mn_major << 15)          // a_major (0 = K, 1 = MN)
-         | ((uint32_t)b_mn_major << 16)          // b_major
-         | ((uint32_t)(N >> 3) << 17)            // n_dim
-         | ((uint32_t)(M >> 4) << 24);           // m_dim
-}
-__host__ __device__ constexpr uint32_t make_idesc_bf16_f32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                       // c_format = F32
-         | (1u << 7)                     // a_format = BF16
-         | (1u << 10)                    // b_format = BF16
-         | ((uint32_t)a_mn_major << 15)  // a_major (0 = K, 1 = MN)
-         | ((uint32_t)b_mn_major << 16)  // b_major
-         | ((uint32_t)(N >> 3) << 17)    // n_dim
-         | ((uint32_t)(M >> 4) << 24);   // m_dim
-}
 
 // ---------------------------------------------------------------- cp.async (LDGSTS)
 __device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gmem_src) {

@@ -38,15 +38,10 @@ int attn_bwd_lse(const void* qkv, const int32_t* attn_mask, const void* ctx, con
                  void* dqkv, float* dbias, int nseq, int S, int heads, float dropout_p,
                  unsigned long long site_seed, cudaStream_t stream);
 
-int attn_fwd_tc(const void* qkv, const int32_t* attn_mask, void* ctx, float* lse, int nseq, int S, int heads,
+int attn_fwd_wg(const void* qkv, const int32_t* attn_mask, void* ctx, float* lse, int nseq, int S, int heads,
                 float dropout_p, unsigned long long site_seed, cudaStream_t stream);
-int attn_fwd_tc2(const void* qkv, const int32_t* attn_mask, void* ctx, float* lse, int nseq, int S, int heads,
-                 float dropout_p, unsigned long long site_seed, cudaStream_t stream);
-int attn_bwd_tc2(const void* qkv, const int32_t* attn_mask, const void* ctx, const float* lse, const void* dctx,
-                 void* dqkv, int nseq, int S, int heads, float dropout_p, unsigned long long site_seed,
-                 cudaStream_t stream);
-int attn_bwd_tc(const void* qkv, const int32_t* attn_mask, const float* lse, const void* dctx, void* dqkv,
-                float* dbias, int nseq, int S, int heads, float dropout_p, unsigned long long site_seed,
+int attn_bwd_wg(const void* qkv, const int32_t* attn_mask, const float* lse, const void* dctx,
+                void* dqkv, int nseq, int S, int heads, float dropout_p, unsigned long long site_seed,
                 cudaStream_t stream);
 
 int attn_cls_fwd(const void* qkv, const int32_t* attn_mask, void* ctx_cls, float* probs, int nseq, int S, int heads,

@@ -85,7 +85,7 @@ ln_fwd_kernel(const bf16* __restrict__ z, const int64_t* __restrict__ ids, const
               bf16* __restrict__ y, bf16* __restrict__ y_res, float* __restrict__ stats, float* __restrict__ cls_out,
               int cls_stride, int T, int H, float eps, Drop drop, int z_f16) {
   // y: bf16 (the next GEMM's A operand, saved for wgrad).  y_res (optional): the same values in fp16 - the copy the
-  // next residual add reads (tcgen05 kind::f16 cannot mix an fp16 operand with bf16 weights, so the stream that must
+  // next residual add reads (a tensor-core MMA cannot mix an fp16 operand with bf16 weights, so the stream that must
   // stay precise travels beside the GEMM operand instead of replacing it).  z_f16: the input sum holds fp16.
   constexpr bool f16 = ZF16;      // compile-time: a run-time format select costs two conversions + a select per pair
   (void)z_f16;
@@ -388,11 +388,9 @@ ln_bwd_kernel(const bf16* __restrict__ dy, const float* __restrict__ dy_cls, int
 
 // ------------------------------------------------------------------ full-width rows: H == MAXC * 256, dense dy
 // The encoder's LayerNorms (H = 768 / 1024, every row has an upstream gradient) take these two kernels.  They do the
-// same arithmetic as ln_fwd_kernel / ln_bwd_kernel on PAIRS of columns with packed fp32 instructions (FADD2 / FMUL2 /
-// FFMA2), without the per-chunk width predicates, and keep gamma / beta in shared memory in a bank-conflict-free
-// layout.  The generic kernels issue 473 (fwd) / 1 132 (bwd) instructions per 768-wide row, more than an SM can issue
-// in the time its share of HBM bandwidth delivers the row (~420 / ~840 issue slots at 6.5 TB/s): they were
-// instruction-bound at ~0.5 of the HBM roofline.
+// same arithmetic as ln_fwd_kernel / ln_bwd_kernel on PAIRS of columns, without the per-chunk width predicates, and
+// keep gamma / beta in shared memory in a bank-conflict-free layout: the generic kernels spend most of their issue
+// slots on those predicates and index computations.
 //
 // Shared-memory layout of a per-column vector v[H] ("pair layout"): chunk i of lane l holds columns c .. c+7 with
 // c = (32 i + l) * 8; columns c..c+3 live at [i*256 + l*4], columns c+4..c+7 at [i*256 + 128 + l*4], so both 16-byte
@@ -435,14 +433,14 @@ ln_fwd_full_kernel(const bf16* __restrict__ z, const float* __restrict__ gamma, 
 #pragma unroll
     for (int i = 0; i < MAXC; ++i)
 #pragma unroll
-      for (int k = 0; k < 4; ++k) s = __fadd2_rn(s, x[i][k]);
+      for (int k = 0; k < 4; ++k) s = fadd2(s, x[i][k]);
     const float mean = warp_sum(s.x + s.y) / (float)H;
     const float2 nm = make_float2(-mean, -mean);
     float2 qq = make_float2(0.f, 0.f);
 #pragma unroll
     for (int i = 0; i < MAXC; ++i)
 #pragma unroll
-      for (int k = 0; k < 4; ++k) { x[i][k] = __fadd2_rn(x[i][k], nm); qq = __ffma2_rn(x[i][k], x[i][k], qq); }
+      for (int k = 0; k < 4; ++k) { x[i][k] = fadd2(x[i][k], nm); qq = ffma2(x[i][k], x[i][k], qq); }
     const float var = warp_sum(qq.x + qq.y) / (float)H;
     const float rstd = rsqrtf(var + eps);
     const float2 r2 = make_float2(rstd, rstd);
@@ -455,7 +453,7 @@ ln_fwd_full_kernel(const bf16* __restrict__ z, const float* __restrict__ gamma, 
       lds8_pairs(s_g, i, lane, g);
       lds8_pairs(s_b, i, lane, b);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) o[k] = __ffma2_rn(__fmul2_rn(x[i][k], r2), g[k], b[k]);
+      for (int k = 0; k < 4; ++k) o[k] = ffma2(fmul2(x[i][k], r2), g[k], b[k]);
       yr[32 * i] = make_uint4(pack_bf16x2(o[0].x, o[0].y), pack_bf16x2(o[1].x, o[1].y), pack_bf16x2(o[2].x, o[2].y),
                               pack_bf16x2(o[3].x, o[3].y));
       if (yres != nullptr)
@@ -539,12 +537,12 @@ ln_bwd_full_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z, cons
       unpack8_pairs(cdy[i], d[i], false);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        xh[i][k] = __fmul2_rn(__fadd2_rn(xh[i][k], nm), r2);
-        ag[i][k] = __ffma2_rn(d[i][k], xh[i][k], ag[i][k]);
-        ab[i][k] = __fadd2_rn(ab[i][k], d[i][k]);
-        d[i][k] = __fmul2_rn(d[i][k], g[k]);       // dxhat
-        s1 = __fadd2_rn(s1, d[i][k]);
-        s2 = __ffma2_rn(d[i][k], xh[i][k], s2);
+        xh[i][k] = fmul2(fadd2(xh[i][k], nm), r2);
+        ag[i][k] = ffma2(d[i][k], xh[i][k], ag[i][k]);
+        ab[i][k] = fadd2(ab[i][k], d[i][k]);
+        d[i][k] = fmul2(d[i][k], g[k]);       // dxhat
+        s1 = fadd2(s1, d[i][k]);
+        s2 = ffma2(d[i][k], xh[i][k], s2);
       }
     }
     const float m1 = warp_sum(s1.x + s1.y) / (float)H;
@@ -558,7 +556,7 @@ ln_bwd_full_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z, cons
       uint32_t w[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        o[k] = __fmul2_rn(r2, __fadd2_rn(__ffma2_rn(xh[i][k], nm2, d[i][k]), nm1));   // rstd * (d - s1 - xh * s2)
+        o[k] = fmul2(r2, fadd2(ffma2(xh[i][k], nm2, d[i][k]), nm1));   // rstd * (d - s1 - xh * s2)
         w[k] = pack_bf16x2(o[k].x, o[k].y);
       }
       dzr[32 * i] = make_uint4(w[0], w[1], w[2], w[3]);
@@ -569,7 +567,7 @@ ln_bwd_full_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z, cons
         drop.mul8((uint32_t)row, (uint32_t)(lane + 32 * i) * 8u, m);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          const float2 om = __fmul2_rn(o[k], m[k]);
+          const float2 om = fmul2(o[k], m[k]);
           w[k] = pack_bf16x2(om.x, om.y);
         }
         dzmr[32 * i] = make_uint4(w[0], w[1], w[2], w[3]);
@@ -578,7 +576,7 @@ ln_bwd_full_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z, cons
         // the Linear's bias gradient: column sums of ITS output gradient (the masked copy when dropout is on), as the
         // bf16-rounded values the downstream GEMMs consume
 #pragma unroll
-        for (int k = 0; k < 4; ++k) az[i][k] = __fadd2_rn(az[i][k], unpack_bf16x2(w[k]));
+        for (int k = 0; k < 4; ++k) az[i][k] = fadd2(az[i][k], unpack_bf16x2(w[k]));
       }
     }
   }
@@ -696,7 +694,7 @@ int ln_fwd(const void* z, const float* gamma, const float* beta, void* y, float*
   if (T == 0) return 0;
   DPRB_REQUIRE(cls_out == nullptr || cls_stride > 0, "ln_fwd: cls_stride must be positive");
   const int grid = grid_for_rows(T);
-  if (H % 256 == 0 && !ln_generic_forced()) {   // full-width rows (the encoder's H = 768 / 1024): packed-fp32 kernel
+  if (H % 256 == 0 && !ln_generic_forced()) {   // full-width rows (the encoder's H = 768 / 1024): paired-column kernel
 #define CALLF(C)                                                                                                         \
   do {                                                                                                                   \
     if (z_f16) ln_fwd_full_kernel<C, true><<<grid, THREADS, 0, stream>>>((const bf16*)z, gamma, beta, (bf16*)y, (bf16*)y_res, stats, cls_out, cls_stride > 0 ? cls_stride : 1, T, eps); \
@@ -729,7 +727,7 @@ int ln_bwd(const void* dy, const float* dy_cls, int cls_stride, const void* z, c
   DPRB_REQUIRE(dy_cls == nullptr || cls_stride > 0, "ln_bwd: cls_stride must be positive");
   const int grid = grid_for_rows(T);
   const int maxc = (H + 255) / 256;
-  if (dy != nullptr && H % 256 == 0 && !ln_generic_forced()) {   // dense upstream gradient, full-width rows: packed-fp32 kernel
+  if (dy != nullptr && H % 256 == 0 && !ln_generic_forced()) {   // dense upstream gradient, full-width rows: paired-column kernel
     size_t front = (size_t)WARPS * H * sizeof(float);
     const size_t ring_f = (size_t)WARPS * PF_DEPTH * (2 * maxc * 512 + 16);
     if (ring_f > front) front = ring_f;

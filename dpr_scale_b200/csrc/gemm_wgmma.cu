@@ -1,0 +1,465 @@
+// bf16 GEMM for sm_90a: TMA -> 128B-swizzled smem ring (mbarrier pipeline) -> wgmma (fp32 accumulators in
+// registers) -> epilogue straight from the accumulator registers, with the fused bias / bias+GELU / bias+residual /
+// dGELU / fp32 split-K accumulate variants the encoder needs.
+//
+// One CTA computes a 128x128 tile: warpgroups 0 and 1 own rows [0, 64) and [64, 128) (wgmma m64n128k16), warp 8 is
+// the TMA producer.  3-stage ring of 32 KB, so two CTAs share an SM and one CTA's epilogue overlaps the other's
+// main loop.
+//
+// Replaces, on the reference path, every torch.nn.Linear call inside HF BertLayer (QKV, attention output,
+// intermediate, output) and their autograd backward (dgrad / wgrad).
+//
+// D[M,N] = epi( sum_k A(m,k) * B(n,k) ).  Each operand may be K-major (row = MN index, K contiguous)
+// or MN-major (row = K index, MN contiguous); the latter lets dgrad read W[N_out,K_in] and wgrad
+// read dY[T,N_out] / X[T,K_in] in place, with no transposed copies.
+#include <cstdlib>
+#include <vector>
+#include "common.cuh"
+#include "dprb_internal.h"
+
+namespace dprb {
+
+namespace {
+
+constexpr int BLOCK_M = 128;
+constexpr int BLOCK_N = 128;
+constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
+constexpr int STAGES = 3;
+constexpr int TILE_BYTES = 128 * BLOCK_K * 2;         // 16 KB: one operand tile of a stage
+constexpr int STAGE_BYTES = 2 * TILE_BYTES;
+constexpr int NUM_CONSUMERS = 2;                      // warpgroups
+constexpr int NUM_THREADS = NUM_CONSUMERS * 128 + 32; // + one producer warp
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 128 /*barriers*/;
+static_assert(2 * SMEM_BYTES <= 227 * 1024, "two CTAs per SM must fit");
+
+struct GemmParams {
+  int M, N, K;
+  int num_m_blocks, num_n_blocks;
+  int k_blocks_total, k_blocks_per_split, splits;
+  int epilogue;
+  void* D;
+  long long ldd;
+  const float* bias;   // [N] fp32 or null
+  const bf16* aux;     // residual (EPI_BIAS_RESIDUAL) or pre-activation (EPI_DGELU), ld = ld_aux
+  long long ld_aux;
+  bf16* out2;          // EPI_BIAS_GELU: pre-activation store, ld = ldd
+  float alpha;         // scale applied to the accumulator before the epilogue
+  float* colsum;       // optional: colsum[n] += sum_m D(m, n) of the bf16-rounded output (bias gradients)
+  Drop drop;           // EPI_BIAS_RESIDUAL only: D = dropout(acc + bias) + aux  (hidden dropout before the residual)
+  int aux_f16, out_f16;  // aux / D hold fp16 instead of bf16 (the encoder's fp16 residual stream)
+  int save_pre;          // EPI_BIAS_GELU: out2 receives the pre-activation itself instead of gelu'(pre) (lean activations)
+};
+
+__device__ __forceinline__ void red_add_v2_f32(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
+
+template <int A_MN, int B_MN, int F16>
+__device__ __forceinline__ void mma_kblock(float (&acc)[64], uint32_t sa, uint32_t sb, int accumulate_first) {
+  // K-major SW128: 8-row groups 1024 B apart; a k16 step is +32 B inside the swizzle row.
+  // MN-major SW128: 64-element MN atoms BLOCK_K*128 B apart (LBO), 8-deep K groups 1024 B apart; a k16 step is
+  // +16 rows of 128 B.
+  const uint64_t da = make_wgmma_desc_sw128(sa, A_MN ? BLOCK_K * 128 : 16, 1024);
+  const uint64_t db = make_wgmma_desc_sw128(sb, B_MN ? BLOCK_K * 128 : 16, 1024);
+  constexpr uint32_t A_KSTEP = (A_MN ? 16 * 128 : 32) >> 4;
+  constexpr uint32_t B_KSTEP = (B_MN ? 16 * 128 : 32) >> 4;
+#pragma unroll
+  for (int k = 0; k < BLOCK_K / 16; ++k) {
+    const int accum = (k > 0 || accumulate_first) ? 1 : 0;
+    if (F16) wgmma_m64n128_ss_f16<A_MN, B_MN>(acc, da + k * A_KSTEP, db + k * B_KSTEP, accum);
+    else wgmma_m64n128_ss_bf16<A_MN, B_MN>(acc, da + k * A_KSTEP, db + k * B_KSTEP, accum);
+  }
+}
+
+__device__ __forceinline__ uint32_t pack_out(float a, float b, bool f16) { return f16 ? pack_f16x2(a, b) : pack_bf16x2(a, b); }
+__device__ __forceinline__ void store_pair(bf16* base, long long off, int col, int N, uint32_t v) {
+  if (col + 1 < N) {
+    *reinterpret_cast<uint32_t*>(base + off) = v;
+  } else if (col < N) {
+    reinterpret_cast<uint16_t*>(base)[off] = (uint16_t)(v & 0xFFFFu);
+  }
+}
+__device__ __forceinline__ float2 load_pair(const bf16* base, long long off, int col, int N, bool f16) {
+  uint32_t u = 0;
+  if (col + 1 < N) u = *reinterpret_cast<const uint32_t*>(base + off);
+  else if (col < N) u = reinterpret_cast<const uint16_t*>(base)[off];
+  return unpack_16x2(u, f16);
+}
+
+template <int A_MN, int B_MN, int F16>
+__global__ void __launch_bounds__(NUM_THREADS, 2)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  // SWIZZLE_128B needs 1024-byte aligned tiles
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                           // [STAGES]
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int tiles = p.num_m_blocks * p.num_n_blocks;
+  const int u = blockIdx.x;
+  const int tile = u % tiles, split = u / tiles;
+  const int m_blk = tile / p.num_n_blocks, n_blk = tile % p.num_n_blocks;
+  const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
+  const int kb0 = split * p.k_blocks_per_split;
+  const int kb1 = min(kb0 + p.k_blocks_per_split, p.k_blocks_total);
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);                   // producer arrive (+ transaction bytes)
+      mbar_init(&empty_bar[i], NUM_CONSUMERS * 4);  // one arrive per consumer warp
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == NUM_CONSUMERS * 4) {
+    // ================================ TMA producer ================================
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
+        uint8_t* sa = smem + stage * STAGE_BYTES;
+        uint8_t* sb = sa + TILE_BYTES;
+        if (A_MN == 0) {
+          tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, m0);
+        } else {
+#pragma unroll
+          for (int i = 0; i < BLOCK_M / 64; ++i) tma_load_2d(sa + i * (BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, kb * BLOCK_K);
+        }
+        if (B_MN == 0) {
+          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, n0);
+        } else {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 64; ++i) tma_load_2d(sb + i * (BLOCK_K * 128), &tmap_b, &full_bar[stage], n0 + i * 64, kb * BLOCK_K);
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+    return;
+  }
+
+  // ================================ consumer warpgroups ================================
+  const int wg = warp >> 2;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  {
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    // this warpgroup's 64 rows of the A tile: K-major +64 rows of 128 B, MN-major the second 64-wide MN atom
+    const uint32_t a_off = (uint32_t)wg * (A_MN ? BLOCK_K * 128 : 64 * 128);
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + a_off;
+      const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES + TILE_BYTES);
+      wgmma_fence();
+      mma_kblock<A_MN, B_MN, F16>(acc, sa, sb, kb > kb0);
+      wgmma_commit();
+      // keep one k-block of MMAs in flight; the one before it has retired and its stage can be refilled
+      wgmma_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+  }
+
+  // ================================ epilogue from registers ================================
+  // thread holds rows r0 (d[4c], d[4c+1]) and r0 + 8 (d[4c+2], d[4c+3]) at columns n0 + 8c + 2q, +1
+  const int q = lane & 3;
+  const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int ep = p.epilogue;
+  const bool f32_out = (ep == DPRB_EPI_F32_ATOMIC_ADD || ep == DPRB_EPI_F32_STORE);
+  if (f32_out) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      if (row >= p.M) continue;
+      float* drow = reinterpret_cast<float*>(p.D) + (long long)row * p.ldd;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        const int col = n0 + 8 * c + 2 * q;
+        const float x = acc[4 * c + 2 * h] * p.alpha, y = acc[4 * c + 2 * h + 1] * p.alpha;
+        if (ep == DPRB_EPI_F32_ATOMIC_ADD) {
+          if (col + 1 < p.N) red_add_v2_f32(drow + col, x, y);
+          else if (col < p.N) atomicAdd(drow + col, x);
+        } else {
+          if (col < p.N) drow[col] = x + (p.bias != nullptr ? __ldg(p.bias + col) : 0.f);
+          if (col + 1 < p.N) drow[col + 1] = y + (p.bias != nullptr ? __ldg(p.bias + col + 1) : 0.f);
+        }
+      }
+    }
+    return;
+  }
+  const bool out_f16 = p.out_f16 != 0;
+  bf16* D = reinterpret_cast<bf16*>(p.D);
+#pragma unroll
+  for (int c = 0; c < 16; ++c) {
+    const int col = n0 + 8 * c + 2 * q;
+    float2 b = make_float2(0.f, 0.f);
+    if (p.bias != nullptr) {
+      if (col + 1 < p.N) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+      else if (col < p.N) b.x = __ldg(p.bias + col);
+    }
+    float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      const bool ok = row < p.M && col < p.N;
+      float2 v = ffma2(make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]), make_float2(p.alpha, p.alpha), b);
+      const long long off = (long long)row * p.ldd + col;
+      if (ep == DPRB_EPI_BIAS_GELU) {
+        float2 g, d;
+        gelu_and_grad2(v, g, d);
+        if (p.save_pre) d = v;        // lean activations: keep pre, rebuild gelu / gelu' in backward
+        if (ok) {
+          if (p.out2 != nullptr) store_pair(p.out2, off, col, p.N, pack_bf16x2(d.x, d.y));
+          store_pair(D, off, col, p.N, pack_bf16x2(g.x, g.y));
+        }
+        continue;
+      }
+      if (ep == DPRB_EPI_BIAS_RESIDUAL && p.drop.on()) {
+        float m0f, m1f;
+        p.drop.mul2((uint32_t)row, (uint32_t)col, m0f, m1f);
+        v.x *= m0f; v.y *= m1f;
+      }
+      if (ep == DPRB_EPI_BIAS_RESIDUAL || ep == DPRB_EPI_DGELU || ep == DPRB_EPI_DGELU_PRE) {
+        const float2 a = ok ? load_pair(p.aux, (long long)row * p.ld_aux + col, col, p.N, p.aux_f16 != 0) : make_float2(0.f, 0.f);
+        if (ep == DPRB_EPI_BIAS_RESIDUAL) {
+          v.x += a.x; v.y += a.y;
+        } else if (ep == DPRB_EPI_DGELU) {
+          v.x *= a.x; v.y *= a.y;       // aux holds gelu'(pre) written by the forward epilogue
+        } else {
+          float2 g, d;                  // aux holds the pre-activation: derivative rebuilt (same fitted function)
+          gelu_and_grad2(a, g, d);
+          v.x *= d.x; v.y *= d.y;
+        }
+      }
+      const uint32_t o = pack_out(v.x, v.y, out_f16);
+      if (ok) {
+        store_pair(D, off, col, p.N, o);
+        if (p.colsum != nullptr) {      // bias gradient: sums of the bf16-rounded output
+          const float2 f = unpack_bf16x2(o);
+          cs0 += f.x;
+          if (col + 1 < p.N) cs1 += f.y;
+        }
+      }
+    }
+    if (p.colsum != nullptr) {
+      // lanes with the same q hold the same columns: reduce over the 8 row groups of the warp
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) {
+        cs0 += __shfl_xor_sync(0xFFFFFFFFu, cs0, o);
+        cs1 += __shfl_xor_sync(0xFFFFFFFFu, cs1, o);
+      }
+      if (lane < 4) {
+        if (col < p.N) atomicAdd(p.colsum + col, cs0);
+        if (col + 1 < p.N) atomicAdd(p.colsum + col + 1, cs1);
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------- host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeTiledFn get_encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  if (fn == nullptr) {
+    void* ptr = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
+        qres != cudaDriverEntryPointSuccess)
+      return nullptr;
+    fn = reinterpret_cast<EncodeTiledFn>(ptr);
+  }
+  return fn;
+}
+
+// Row-major bf16 matrix [rows, cols] with leading dimension ld (elements); box = [box_rows, 64 cols], 128B swizzle.
+int make_tmap(CUtensorMap* out, const void* base, long long rows, long long cols, long long ld, int box_rows) {
+  static thread_local bool ctx_bound = false;   // driver entry point: needs a current context on THIS thread
+  if (!ctx_bound) {
+    DPRB_CHECK_CUDA(cudaFree(nullptr));
+    ctx_bound = true;
+  }
+  EncodeTiledFn fn = get_encode_fn();
+  DPRB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  DPRB_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "gemm operand base %p not 16-byte aligned", base);
+  DPRB_REQUIRE((ld * 2) % 16 == 0, "gemm operand leading dimension %lld not a multiple of 8 elements", ld);
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1u, 1u};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  DPRB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (rows=%lld cols=%lld ld=%lld)",
+               (int)r, rows, cols, ld);
+  return 0;
+}
+
+// ---- optional live profiling: CUDA events around every GEMM launch (bench.py's roofline leg) ----
+struct GemmProfile {
+  bool enabled = false;
+  std::vector<cudaEvent_t> ev;   // pairs
+  std::vector<double> flops;
+  size_t used = 0;
+};
+GemmProfile g_prof;
+
+int choose_splits(int tiles, int k_blocks, int sms) {
+  // minimise the makespan ceil(tiles*s/sms)/s over s, keeping >= 4 k-blocks per split
+  int best = 1;
+  double best_cost = 1e30;
+  for (int s = 1; s <= 32; ++s) {
+    if (k_blocks / s < 4 && s > 1) break;
+    int waves = (tiles * s + sms - 1) / sms;
+    double cost = (double)waves / s + 0.002 * s;  // small penalty for extra atomic traffic
+    if (cost < best_cost - 1e-9) { best_cost = cost; best = s; }
+  }
+  return best;
+}
+
+}  // namespace
+
+int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long long lda, long long ldb,
+              long long ldd, int a_mn_major, int b_mn_major, int epilogue, const float* bias, const void* aux,
+              long long ld_aux, void* out2, float alpha, int splits, float* colsum, float dropout_p,
+              unsigned long long drop_site_seed, cudaStream_t stream) {
+  DPRB_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
+  const int dt_flags = epilogue & ~0xFF;   // DPRB_GEMM_{A,B,AUX,OUT}_F16, DPRB_GEMM_SAVE_PRE
+  epilogue &= 0xFF;
+  const int a_f16 = (dt_flags & DPRB_GEMM_A_F16) != 0, b_f16 = (dt_flags & DPRB_GEMM_B_F16) != 0;
+  const int aux_f16 = (dt_flags & DPRB_GEMM_AUX_F16) != 0, out_f16 = (dt_flags & DPRB_GEMM_OUT_F16) != 0;
+  DPRB_REQUIRE(epilogue >= 0 && epilogue < DPRB_EPI_COUNT, "gemm: bad epilogue %d", epilogue);
+  DPRB_REQUIRE(!(aux_f16 || out_f16) || epilogue == DPRB_EPI_BIAS || epilogue == DPRB_EPI_BIAS_RESIDUAL,
+               "gemm: fp16 aux / output is implemented for the BIAS and BIAS_RESIDUAL epilogues only");
+  DPRB_REQUIRE(a_f16 == b_f16, "gemm: wgmma takes no fp16 x bf16 operand pair: give "
+               "DPRB_GEMM_A_F16 and DPRB_GEMM_B_F16 together or not at all");
+  DPRB_REQUIRE(!out_f16 || colsum == nullptr, "gemm: colsum reads a bf16 slab (not available with fp16 output)");
+  const bool f32_out = (epilogue == DPRB_EPI_F32_ATOMIC_ADD || epilogue == DPRB_EPI_F32_STORE);
+  DPRB_REQUIRE(f32_out || (ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0),
+               "gemm: bf16 output must be 16-byte aligned with ldd %% 8 == 0 (ldd=%lld)", ldd);
+  DPRB_REQUIRE(!f32_out || (ldd % 4 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0),
+               "gemm: fp32 output must be 16-byte aligned with ldd %% 4 == 0 (ldd=%lld)", ldd);
+  if (epilogue == DPRB_EPI_BIAS_RESIDUAL || epilogue == DPRB_EPI_DGELU || epilogue == DPRB_EPI_DGELU_PRE)
+    DPRB_REQUIRE(aux != nullptr && ld_aux % 8 == 0, "gemm: epilogue %d needs aux with ld %% 8 == 0", epilogue);
+  if (bias != nullptr) DPRB_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "gemm: bias not 16B aligned");
+
+  DPRB_REQUIRE(colsum == nullptr || (!f32_out && epilogue != DPRB_EPI_BIAS_GELU),
+               "gemm: colsum is supported for the BIAS / BIAS_RESIDUAL / DGELU epilogues only");
+
+  CUtensorMap ta, tb;
+  int rc;
+  if (!a_mn_major) rc = make_tmap(&ta, A, M, K, lda, BLOCK_M); else rc = make_tmap(&ta, A, K, M, lda, BLOCK_K);
+  if (rc) return rc;
+  if (!b_mn_major) rc = make_tmap(&tb, B, N, K, ldb, BLOCK_N); else rc = make_tmap(&tb, B, K, N, ldb, BLOCK_K);
+  if (rc) return rc;
+
+  GemmParams p;
+  p.M = M; p.N = N; p.K = K;
+  p.num_m_blocks = (M + BLOCK_M - 1) / BLOCK_M;
+  p.num_n_blocks = (N + BLOCK_N - 1) / BLOCK_N;
+  p.k_blocks_total = (K + BLOCK_K - 1) / BLOCK_K;
+  const int sms = num_sms();
+  const int tiles = p.num_m_blocks * p.num_n_blocks;
+  if (epilogue != DPRB_EPI_F32_ATOMIC_ADD) splits = 1;
+  else if (splits <= 0) splits = choose_splits(tiles, p.k_blocks_total, 2 * sms);   // two CTAs per SM
+  if (splits > p.k_blocks_total) splits = p.k_blocks_total;
+  p.k_blocks_per_split = (p.k_blocks_total + splits - 1) / splits;
+  p.splits = (p.k_blocks_total + p.k_blocks_per_split - 1) / p.k_blocks_per_split;
+  p.epilogue = epilogue;
+  p.D = D; p.ldd = ldd; p.bias = bias; p.aux = reinterpret_cast<const bf16*>(aux); p.ld_aux = ld_aux;
+  p.out2 = reinterpret_cast<bf16*>(out2); p.alpha = alpha;
+  p.colsum = colsum;
+  p.aux_f16 = aux_f16; p.out_f16 = out_f16;
+  p.save_pre = (dt_flags & DPRB_GEMM_SAVE_PRE) != 0;
+  p.drop = drop_from_site(epilogue == DPRB_EPI_BIAS_RESIDUAL ? dropout_p : 0.f, drop_site_seed);
+  if (epilogue == DPRB_EPI_BIAS_GELU && out2 != nullptr)
+    DPRB_REQUIRE((reinterpret_cast<uintptr_t>(out2) & 15) == 0, "gemm: out2 not 16-byte aligned");
+
+  const int grid = tiles * p.splits;
+  static bool attr_set = false;
+  if (!attr_set) {
+#define DPRB_SET_ATTR(...) DPRB_CHECK_CUDA(cudaFuncSetAttribute(__VA_ARGS__, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    DPRB_SET_ATTR(gemm_bf16_kernel<0, 0, 0>) DPRB_SET_ATTR(gemm_bf16_kernel<0, 1, 0>)
+    DPRB_SET_ATTR(gemm_bf16_kernel<1, 0, 0>) DPRB_SET_ATTR(gemm_bf16_kernel<1, 1, 0>)
+    DPRB_SET_ATTR(gemm_bf16_kernel<0, 0, 1>) DPRB_SET_ATTR(gemm_bf16_kernel<0, 1, 1>)
+    DPRB_SET_ATTR(gemm_bf16_kernel<1, 0, 1>) DPRB_SET_ATTR(gemm_bf16_kernel<1, 1, 1>)
+#undef DPRB_SET_ATTR
+    attr_set = true;
+  }
+  auto launch = [&](auto kern) -> int {
+    const bool prof = g_prof.enabled && g_prof.used + 2 <= g_prof.ev.size();
+    if (prof) DPRB_CHECK_CUDA(cudaEventRecord(g_prof.ev[g_prof.used], stream));
+    kern<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p);
+    DPRB_LAUNCH_CHECK();
+    if (prof) {
+      DPRB_CHECK_CUDA(cudaEventRecord(g_prof.ev[g_prof.used + 1], stream));
+      g_prof.flops.push_back(2.0 * (double)M * (double)N * (double)K);
+      g_prof.used += 2;
+    }
+    return 0;
+  };
+  const int key = (a_mn_major ? 4 : 0) | (b_mn_major ? 2 : 0) | (a_f16 ? 1 : 0);
+  switch (key) {
+    case 0: return launch(gemm_bf16_kernel<0, 0, 0>);
+    case 1: return launch(gemm_bf16_kernel<0, 0, 1>);
+    case 2: return launch(gemm_bf16_kernel<0, 1, 0>);
+    case 3: return launch(gemm_bf16_kernel<0, 1, 1>);
+    case 4: return launch(gemm_bf16_kernel<1, 0, 0>);
+    case 5: return launch(gemm_bf16_kernel<1, 0, 1>);
+    case 6: return launch(gemm_bf16_kernel<1, 1, 0>);
+    default: return launch(gemm_bf16_kernel<1, 1, 1>);
+  }
+}
+
+int gemm_profile_enable(int enable, int max_launches) {
+  if (enable) {
+    const size_t want = (size_t)max_launches * 2;
+    while (g_prof.ev.size() < want) {
+      cudaEvent_t e;
+      DPRB_CHECK_CUDA(cudaEventCreate(&e));
+      g_prof.ev.push_back(e);
+    }
+    g_prof.used = 0;
+    g_prof.flops.clear();
+  }
+  g_prof.enabled = enable != 0;
+  return 0;
+}
+
+// Sums the recorded launch durations (synchronises on each end event). Outputs: total ms, total FLOPs, launches.
+int gemm_profile_read(double* total_ms, double* total_flops, long long* launches) {
+  double ms = 0.0, fl = 0.0;
+  for (size_t i = 0; i + 1 < g_prof.used; i += 2) {
+    DPRB_CHECK_CUDA(cudaEventSynchronize(g_prof.ev[i + 1]));
+    float t = 0.f;
+    DPRB_CHECK_CUDA(cudaEventElapsedTime(&t, g_prof.ev[i], g_prof.ev[i + 1]));
+    ms += t;
+    fl += g_prof.flops[i / 2];
+  }
+  if (total_ms) *total_ms = ms;
+  if (total_flops) *total_flops = fl;
+  if (launches) *launches = (long long)(g_prof.used / 2);
+  return 0;
+}
+
+}  // namespace dprb

@@ -6,7 +6,7 @@
 // :211 (scores /= temperature), :212 (nn.CrossEntropyLoss) and, for the multi-rank case, the gradient
 // flow implied by :163-195 (remote slices are detached; only local rows/columns get gradients).
 //
-// All arithmetic is fp32 (the reference under AMP does this product in fp16 — SURVEY §8a7); the work
+// All arithmetic is fp32 (the reference under AMP does this product in fp16); the work
 // is 2*Q*C*d FLOP = 0.2 GFLOP (cfg 2) .. 12.9 GFLOP (cfg 3), latency-bound, so it stays on the FFMA pipe.
 #include "common.cuh"
 #include "dprb_internal.h"

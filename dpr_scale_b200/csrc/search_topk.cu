@@ -1,19 +1,19 @@
-// Brute-force inner-product search with a running top-k, for sm_100a.
+// Brute-force inner-product search with a running top-k, for sm_90a.
 //
-// Replaces search_index() of the reference (/root/reference/dpr_scale/run_retrieval_pytorch.py:141-176):
+// Replaces search_index() of the reference (dpr_scale/run_retrieval_pytorch.py):
 //     scores = einsum('ik,jk->ij', queries.half(), corpus)          # [Q, N] fp16, materialised
 //     sort_scores, sort_candidates = torch.topk(scores, k)          # several more passes over [Q, N]
-// and the per-shard merge of :210-230 / :272-277 (concat shard results, topk, gather).
+// and the per-shard merge (concat shard results, topk, gather).
 //
-// B200 design: the [Q, N] score matrix never exists.  The corpus ([N, d] fp16/bf16, K-major, resident in HBM) is
-// streamed ONCE per block of <= 128 queries through a TMA -> tcgen05 pipeline (UMMA 128x256x16, fp32 accumulators
-// in TMEM, double buffered).  The accumulator's row-per-lane layout makes every filter thread the owner of one
-// query: it keeps that query's current bar in a register, tests the max of each 32-score chunk against it, and
+// Design: the [Q, N] score matrix never exists.  The corpus ([N, d] fp16/bf16, K-major, resident in HBM) is
+// streamed ONCE per block of <= 128 queries through a TMA -> wgmma pipeline (two m64n128k16 per k16 step, fp32
+// accumulators staged in shared memory as a [128 query][128 row] tile).  Thread i of the filter warpgroup owns
+// query i: it keeps that query's current bar in a register, tests the max of each 32-score chunk against it, and
 // appends the (rare) scores above the bar to a private candidate queue.  The bar is the larger of the query's own
 // k-th best (a full queue is cut back to its best k by the whole warp: exact bisection on (score, ~row) keys) and
 // a cross-partition bound (min over partitions of their m-th best, m = ceil(k / partitions)), which rises much
-// faster and keeps the queues a few entries long.  The kernel is HBM-bound on the corpus stream: 2*d bytes per
-// corpus row per query block (measured 6.0-6.7 TB/s).  A second small kernel merges the per-CTA queues of every
+// faster and keeps the queues a few entries long.  The corpus stream costs 2*d bytes per corpus row per query
+// block.  A second small kernel merges the per-CTA queues of every
 // query (exact selection + bitonic sort).
 //
 // Ranking is by fp32-accumulated score, ties broken towards the lower index (torch.topk leaves tie order
@@ -29,18 +29,18 @@ namespace {
 
 typedef unsigned long long u64;
 
-constexpr int QT = 128;       // queries per CTA = TMEM lanes
-constexpr int CT = 256;       // corpus rows per tile = UMMA N
+constexpr int QT = 128;       // queries per CTA = filter threads
+constexpr int CT = 128;       // corpus rows per tile = wgmma N
 constexpr int BK = 64;        // 64 x 2 B = one 128-byte swizzle row
 constexpr int UK = 16;
 constexpr int STAGES = 4;
 constexpr int A_BYTES = QT * BK * 2;   // 16 KB
-constexpr int B_BYTES = CT * BK * 2;   // 32 KB
+constexpr int B_BYTES = CT * BK * 2;   // 16 KB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int ACC = 2;
-constexpr int TMEM_COLS = ACC * CT;    // 512
-constexpr int THREADS = 256;           // warp 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4-7 filter
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
+constexpr int ACC_LD = CT + 4;         // fp32 score tile [QT][ACC_LD] (padded: conflict-free row reads)
+constexpr int THREADS = 256;           // warp 0 TMA, warps 4-7 (warpgroup 1) wgmma + filter
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + QT * ACC_LD * 4 + 1024 + 256;
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget exceeded");
 constexpr int MAX_QTILES = 8;          // query tiles per launch (they share the corpus stream through L2)
 
 constexpr int SEL_THREADS = 1024;
@@ -59,7 +59,7 @@ struct SearchParams {
   uint32_t* bounds;     // [gridDim.x][gridDim.y * 128] ordered-uint of each partition's m-th best score (0 = none yet)
   int m_track;          // m = ceil(k / partitions) if <= 8, else 0 (cross-partition bound disabled)
   int pf_ahead;         // corpus k-block boxes prefetched into L2 ahead of the shared-memory ring (0 = off)
-  uint32_t idesc;
+  int f16;              // operands are fp16 (else bf16)
   int rank_f16;         // rank by the fp16-ROUNDED score: the reference's einsum on fp16 tensors returns fp16
                         // (run_retrieval_pytorch.py:150-151), so its topk orders fp16 values; ties go to the lower row id
 };
@@ -163,12 +163,10 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  float* sAcc = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [QT][ACC_LD]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + QT * ACC_LD);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full_bar = bars + 2 * STAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + ACC;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + ACC);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -183,25 +181,17 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < ACC; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 4);
+      mbar_init(&empty_bar[i], 4);   // one arrive per filter warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_base_slot, TMEM_COLS);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
   if (warp == 0) {
     // ---------------- TMA producer: query tile (L2-resident) + corpus tile (HBM stream) per k-block
     if (lane == 0) {
-      // Optional: pull corpus boxes into L2 pf_ahead k-blocks ahead of the 4-stage ring (DPRB_SEARCH_PF; measured
-      // slower than the plain ring on B200, so off by default).
+      // Optional: pull corpus boxes into L2 pf_ahead k-blocks ahead of the 4-stage ring (DPRB_SEARCH_PF; off by
+      // default).
       int stage = 0;
       uint32_t phase = 0;
       const long long items = (t1 - t0) * p.kblocks;
@@ -228,36 +218,8 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ---------------- MMA issuer
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (long long t = t0; t < t1; ++t) {
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * CT;
-        for (int kb = 0; kb < p.kblocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint64_t a_desc = make_umma_desc_sw128(smem_u32(smem_a + stage * A_BYTES), 0, 1024);
-          const uint64_t b_desc = make_umma_desc_sw128(smem_u32(smem_b + stage * B_BYTES), 0, 1024);
-#pragma unroll
-          for (int k = 0; k < BK / UK; ++k)
-            umma_f16(d_tmem, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), p.idesc,
-                     (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full_bar[acc]);
-        if (++acc == ACC) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-    __syncwarp();
   } else if (warp >= 4) {
-    // ---------------- threshold filter: thread <-> TMEM lane <-> query
+    // ---------------- wgmma + threshold filter: thread <-> query
     const int quarter = warp & 3;
     const int qslot = blockIdx.y * QT + quarter * 32 + lane;         // < gridDim.y * 128
     const int qpad = gridDim.y * QT;
@@ -277,13 +239,47 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
     uint32_t* my_bound = p.bounds + (size_t)blockIdx.x * qpad + qslot;
     const uint32_t* q_bounds = p.bounds + qslot;
     float lowbar = fminf(thr, t7_);
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
     long long done = 0;
+    const float* arow = sAcc + (quarter * 32 + lane) * ACC_LD;
     for (long long t = t0; t < t1; ++t) {
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tcgen05_fence_after();
-      const uint32_t tbase = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * CT);
+      {
+        float d0[64], d1[64];      // query rows [0, 64) and [64, 128) of the tile
+        for (int kb = 0; kb < p.kblocks; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint64_t a_desc = make_wgmma_desc_sw128(smem_u32(smem_a + stage * A_BYTES), 16, 1024);
+          const uint64_t b_desc = make_wgmma_desc_sw128(smem_u32(smem_b + stage * B_BYTES), 16, 1024);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / UK; ++k) {
+            const int accum = (kb > 0 || k > 0) ? 1 : 0;
+            if (p.f16) {
+              wgmma_m64n128_ss_f16<0, 0>(d0, a_desc + 2 * k, b_desc + 2 * k, accum);
+              wgmma_m64n128_ss_f16<0, 0>(d1, a_desc + 64 * 8 + 2 * k, b_desc + 2 * k, accum);   // +64 rows of 128 B
+            } else {
+              wgmma_m64n128_ss_bf16<0, 0>(d0, a_desc + 2 * k, b_desc + 2 * k, accum);
+              wgmma_m64n128_ss_bf16<0, 0>(d1, a_desc + 64 * 8 + 2 * k, b_desc + 2 * k, accum);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        // the previous tile's rows have all been read (barrier at the end of the loop body)
+        const int r0 = quarter * 16 + (lane >> 2), q4 = lane & 3;
+#pragma unroll
+        for (int c = 0; c < CT / 8; ++c) {
+          float* a0 = sAcc + r0 * ACC_LD + 8 * c + 2 * q4;
+          *reinterpret_cast<float2*>(a0) = make_float2(d0[4 * c], d0[4 * c + 1]);
+          *reinterpret_cast<float2*>(a0 + 8 * ACC_LD) = make_float2(d0[4 * c + 2], d0[4 * c + 3]);
+          *reinterpret_cast<float2*>(a0 + 64 * ACC_LD) = make_float2(d1[4 * c], d1[4 * c + 1]);
+          *reinterpret_cast<float2*>(a0 + 72 * ACC_LD) = make_float2(d1[4 * c + 2], d1[4 * c + 3]);
+        }
+      }
+      asm volatile("bar.sync 1, 128;" ::: "memory");
       const long long rem = p.N - t * CT;
       const int ncols = rem < CT ? (int)rem : CT;
       const uint32_t idx0 = (uint32_t)(t * CT);
@@ -295,8 +291,8 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
           lowbar = fminf(thr, t7_);
         }
         uint32_t r[32];
-        tmem_ld_32x32(tbase + c * 32, r);
-        tmem_ld_wait();
+#pragma unroll
+        for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(r + j) = *reinterpret_cast<const float4*>(arow + c * 32 + j);
         const uint32_t ib = idx0 + c * 32;
         const int nvalid = ncols - c * 32;          // >= 32 except in the ragged last tile
         // one test per 32 scores: in steady state almost no chunk holds a score above the bar
@@ -327,10 +323,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
           }
         }
       }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-      if (++acc == ACC) { acc = 0; acc_phase ^= 1; }
+      asm volatile("bar.sync 1, 128;" ::: "memory");   // the tile is read: the next one may overwrite it
       ++done;
       if (p.m_track > 0 && ((done & (done - 1)) == 0 || (done & 31) == 0)) {
         const int mt = p.m_track;
@@ -358,12 +351,6 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
     p.counts[(size_t)blockIdx.x * qpad + qslot] = (int)cnt;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // One CTA per query: gather the candidate lists, select the k best keys exactly, sort them, write scores / indices.
@@ -498,11 +485,6 @@ int make_tmap(CUtensorMap* out, const void* base, long long rows, int d, int box
   return 0;
 }
 
-constexpr uint32_t make_idesc16(int M, int N, int fmt /*0 = f16, 1 = bf16*/) {
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-
 int num_sms_cached() {
   static int sms = 0;
   if (sms == 0) {
@@ -609,7 +591,7 @@ int search_topk(const void* queries, const void* corpus, int dtype, long long Q,
     SearchParams sp;
     sp.N = N; sp.Q = Qb; sp.d = d; sp.k = k; sp.kblocks = (d + BK - 1) / BK;
     sp.tiles = tiles; sp.tiles_per_part = tpp; sp.queues = queues; sp.counts = counts;
-    sp.idesc = make_idesc16(QT, CT, dtype);
+    sp.f16 = dtype == 0 ? 1 : 0;
     sp.rank_f16 = rank_f16;
     const long long m = (k + parts - 1) / parts;
     sp.bounds = bounds;

@@ -1,10 +1,10 @@
-"""Input pipeline for the training step (SURVEY.md section 8f row 4) with the interface of the reference's
+"""Input pipeline for the training step with the interface of the reference's
 ``dpr_scale.datamodule.dpr.DenseRetrieverJsonlDataModule`` (/root/reference/dpr_scale/datamodule/dpr.py:263-331,
 loaders :178-216) and ``MemoryMappedDataset`` (:23-53).
 
 What the reference does per step, on the training thread with ``num_workers: 0``: seek + readline for every row, ujson
-parse, negative sampling, tokenise ~(2+n)·B sequences, then a blocking H2D copy inside the step.  At B200 step times
-(88 ms for 128 queries + 1024 contexts) that serial CPU work is longer than the GPU work.  Here:
+parse, negative sampling, tokenise ~(2+n)·B sequences, then a blocking H2D copy inside the step.  At the GPU step times of
+this path (tens of ms for 128 queries + 1024 contexts) that serial CPU work is longer than the GPU work.  Here:
 
   * ``LineFile``: the JSONL file is mmap'ed once and its line offsets are found with a vectorised newline scan
     (numpy over the mapping, 64 MB at a time) instead of a Python readline loop; rows are zero-copy slices.
@@ -363,7 +363,7 @@ class DenseRetrieverJsonlDataModule(DenseRetrieverDataModuleBase):
                  **kwargs):
         super().__init__(transform)
         if use_cross_attention:
-            raise NotImplementedError("cross-attention transform is outside the bi-encoder path (DESIGN.md section 0)")
+            raise NotImplementedError("cross-attention transform is outside the bi-encoder path (only the bi-encoder step is implemented)")
         self.batch_size = batch_size
         self.val_batch_size = val_batch_size if val_batch_size else batch_size
         self.test_batch_size = test_batch_size if test_batch_size else self.val_batch_size

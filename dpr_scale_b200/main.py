@@ -18,7 +18,7 @@ from .utils.config import compose, instantiate
 def init_distributed():
     """One process per GPU under torchrun: bind the device and join the NCCL group BEFORE the Trainer reads the world
     size (what Lightning's DDP strategy does inside `Trainer.fit`, main.py:32-44 of the reference).  Without it every
-    rank would train alone on cuda:0 (ADVICE r1)."""
+    rank would train alone on cuda:0."""
     from .utils.dist_init import init_process_group
     return init_process_group()
 

@@ -1,5 +1,5 @@
 """HFEncoder — drop-in for ``dpr_scale.models.hf_model.HFEncoder`` (/root/reference/dpr_scale/models/hf_model.py:12-41)
-whose transformer arithmetic runs entirely in libdprb.so (hand-written sm_100a kernels).
+whose transformer arithmetic runs entirely in libdprb.so (hand-written sm_90a kernels).
 
 Same constructor kwargs (``model_path, dropout, projection_dim``), same call signature
 (``forward(tokens: Mapping) -> Tensor[N, d]``, fresh storage like the reference's ``.clone()``), same
@@ -139,7 +139,7 @@ class _EncoderFn(torch.autograd.Function):
         ctx.state = None
         try:
             # shared_model=True: the same encoder back-propagates twice per step into one gradient arena; only the
-            # LAST outstanding backward may hand finished slices to the trainer's all-reduce (ADVICE r1, trainer.py)
+            # LAST outstanding backward may hand finished slices to the trainer's all-reduce (trainer.py)
             enc._run_backward(state, dpooled.contiguous().float(), sync=enc._pending_bwd <= 1)
         finally:
             enc._pending_bwd = max(0, enc._pending_bwd - 1)
@@ -187,7 +187,7 @@ class _ChunkedEncoderFn(torch.autograd.Function):
 
 class _ProjectFn(torch.autograd.Function):
     """``project = Sequential(Linear(H, p), LayerNorm(p))`` of hf_model.py:26-34 on the dprb kernels:
-    pooled fp32 -> bf16 -> tcgen05 GEMM (+bias, bf16 out) -> dprb_ln_fwd whose fp32 row output IS the result;
+    pooled fp32 -> bf16 -> wgmma GEMM (+bias, bf16 out) -> dprb_ln_fwd whose fp32 row output IS the result;
     backward: dprb_ln_bwd (fused dgamma / dbeta / Linear-bias gradient) -> wgrad GEMM (fp32 split-K accumulate) and
     dgrad GEMM (fp32 store) back into the encoder's upstream gradient.  Same precision contract as the encoder body:
     16-bit GEMM operands, fp32 accumulation, fp32 LayerNorm statistics, fp32 parameters and gradients."""
@@ -229,7 +229,7 @@ class _FwdState:
     """What one forward hands to its backward: the C structs, the token tensors they point into, and a LEASE on the
     activation workspace.  The workspace goes back to the encoder's pool when the state is released (end of backward)
     or garbage-collected (a forward whose graph is dropped) - never while a backward may still read it, so two live
-    forwards of one encoder (shared_model=True: query + context pass of equal shape) cannot alias (VERDICT r1)."""
+    forwards of one encoder (shared_model=True: query + context pass of equal shape) cannot alias."""
 
     __slots__ = ("w", "b", "keep", "ws", "_pool")
 
@@ -287,7 +287,7 @@ class _Transformer(nn.Module):
         self.pooler.add_module("dense", nn.Linear(H, H))
         # Checkpoints written with the reference's pinned transformers==3.4.0 carry the persistent buffer
         # `embeddings.position_ids` (later releases made it non-persistent); it holds arange(max_pos) and is not a
-        # weight, so it is dropped on load instead of failing a strict load_state_dict (ADVICE r1).
+        # weight, so it is dropped on load instead of failing a strict load_state_dict.
         self._register_load_state_dict_pre_hook(self._drop_position_ids)
 
     @staticmethod
@@ -428,7 +428,7 @@ class HFEncoder(nn.Module):
         t = self.transformer
         m = t._master
         if not m.is_cuda:
-            raise _lib.DprbError("HFEncoder (dprb) runs on CUDA only — move the module to a B200 (`.cuda()`); "
+            raise _lib.DprbError("HFEncoder (dprb) runs on CUDA only — move the module to an H100 (`.cuda()`); "
                                  "there is no CPU fallback")
         if t._shadow is None or t._shadow.device != m.device:
             t.__dict__["_shadow"] = torch.empty(m.numel(), dtype=torch.bfloat16, device=m.device)

@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C ABI (raw device pointers + the current CUDA stream).
 
 PyTorch is plumbing here: device memory, streams, autograd bookkeeping.  Every function launches
-hand-written sm_100a kernels from libdprb.so; nothing falls back to torch math.
+hand-written sm_90a kernels from libdprb.so; nothing falls back to torch math.
 """
 import torch
 

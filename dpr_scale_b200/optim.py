@@ -1,5 +1,5 @@
 """FusedAdamW — torch.optim.AdamW semantics (conf/task/optim/adamw.yaml of the reference) executed by ONE
-sm_100a kernel per encoder arena: global-norm clip (Lightning's ``gradient_clip_val``,
+sm_90a kernel per encoder arena: global-norm clip (Lightning's ``gradient_clip_val``,
 conf/trainer/gpu_1_host.yaml:8) + decoupled-weight-decay Adam + bf16 shadow refresh, no host sync.
 
 It is a ``torch.optim.Optimizer`` so ``LambdaLR`` (dpr_task.py:144) drives ``param_groups[0]['lr']`` unchanged.

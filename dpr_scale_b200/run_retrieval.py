@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
-"""Brute-force retrieval over the ``reps_*`` files written by GenerateEmbeddingsTask - the B200 counterpart of
+"""Brute-force retrieval over the ``reps_*`` files written by GenerateEmbeddingsTask - the GPU counterpart of
 /root/reference/dpr_scale/run_retrieval_pytorch.py (same command line, same output files).
 
 What changes under the hood:
-  * search_index (:141-176) is ONE fused kernel pass per 1024 queries (ops.search_topk: tcgen05 scoring with a
+  * search_index (:141-176) is ONE fused kernel pass per 1024 queries (ops.search_topk: wgmma scoring with a
     running top-k); the [batch, N] fp16 score matrix and the torch.topk passes over it are gone, so ``--batch`` no
     longer bounds memory (it is accepted and ignored).
-  * an index segment is held in HBM as fp16 exactly like build_index (:178-190); with 180 GB per GPU the 21 M x 768
+  * an index segment is held in HBM as fp16 exactly like build_index (:178-190); with 80 GB per GPU the 21 M x 768
     Wikipedia index (32 GB) is one segment.  ``--shard`` still splits the reps_* files into sequential segments and
     the per-segment lists are merged on the GPU (ops.topk_merge, replacing :210-230 / :272-277).
   * scores are rounded to fp16 before they are written, because the reference's scores are fp16 einsum outputs;

@@ -3,7 +3,7 @@
 /root/reference/dpr_scale/task/dpr_eval_task.py (:13-49 and :52-84): same constructor keywords, same Lightning test
 hooks, same output files (pickle protocol 4 of ONE fp32 CPU tensor, which is what run_retrieval reads).
 
-How a B200 changes the loop: the encoder runs in its forward-only mode (two activation slots instead of one per layer),
+How this path changes the loop: the encoder runs in its forward-only mode (two activation slots instead of one per layer),
 every batch result goes to one of a few pinned host buffers with an asynchronous copy instead of the reference's blocking
 ``.cpu()`` per batch, and the rows are appended to the pickle's payload as their copies land
 (utils/reps_writer.StreamingTensorPickle) - the shard is never held in RAM, where the reference holds it twice

@@ -1,5 +1,5 @@
 """DenseRetrieverTask — drop-in for ``dpr_scale.task.dpr_task.DenseRetrieverTask``
-(/root/reference/dpr_scale/task/dpr_task.py:17-368) with the arithmetic on hand-written sm_100a kernels.
+(/root/reference/dpr_scale/task/dpr_task.py:17-368) with the arithmetic on hand-written sm_90a kernels.
 
 Same constructor kwargs, same Lightning hook names (``setup``, ``training_step``, ``validation_step`` /
 ``_epoch_end``, ``test_step`` / ``_epoch_end``, ``configure_optimizers``, ``on_load_checkpoint``,

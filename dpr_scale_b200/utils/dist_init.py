@@ -1,10 +1,9 @@
 """Process-group set-up shared by the entry points (main, generate_embeddings, run_retrieval, bench.py).
 
 One process per GPU, NCCL over NVLink / NVSwitch.  The NCCL stream is created with HIGH priority: the gradient
-all-reduce is issued bucket by bucket during backward, whose persistent tcgen05 GEMMs fill every SM; a normal-priority
+all-reduce is issued bucket by bucket during backward, whose GEMMs fill every SM; a normal-priority
 NCCL kernel only gets its ~24 CTAs at the next kernel boundary and in competition with the next GEMM's CTAs, so the
-buckets queue up and ~3.4 ms of all-reduce were still outstanding when backward ended (8 x B200, phases in
-profiles/).  With priority its CTAs are placed as soon as any CTA retires.
+buckets queue up and part of the all-reduce is still outstanding when backward ends.  With priority its CTAs are placed as soon as any CTA retires.
 """
 import os
 

@@ -1,7 +1,7 @@
 """Per-phase device timing of a training step with CUDA events on the launching stream (no host synchronisation inside
 the step).  The trainer and the task call ``mark(name)`` at phase boundaries when a timer is attached; the time between
 two consecutive marks is attributed to the LATER mark's name.  Used by bench.py to say what the multi-GPU step spends
-outside the GEMMs (gather, scoring, exposed gradient all-reduce wait, optimizer) - VERDICT r1, item 6."""
+outside the GEMMs (gather, scoring, exposed gradient all-reduce wait, optimizer)."""
 import collections
 
 import torch

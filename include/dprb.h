@@ -1,4 +1,4 @@
-/* dprb.h — C ABI of libdprb.so: the B200 (sm_100a) drop-in for the arithmetic of dpr-scale's
+/* dprb.h — C ABI of libdprb.so: the H100 (sm_90a) drop-in for the arithmetic of dpr-scale's
  * bi-encoder contrastive training step.
  *
  * The reference (facebookresearch/dpr-scale) is pure Python and has no FFI of its own; every FLOP on
@@ -37,7 +37,7 @@ int dprb_num_sms(void);
 int64_t dprb_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------
- * GEMM (tcgen05 / TMA / TMEM):  D[M,N] = epilogue( alpha * sum_k A(m,k) * B(n,k) )
+ * GEMM (TMA / wgmma):  D[M,N] = epilogue( alpha * sum_k A(m,k) * B(n,k) )
  * Replaces torch.nn.Linear forward/backward inside HF BertLayer:
  *   site-packages/transformers/models/bert/modeling_bert.py:179-181 (Q,K,V — fused here into one
  *   [3H,H] weight), :295 (attention output dense), :340 (intermediate dense), :353 (output dense).
@@ -59,8 +59,8 @@ enum {
   DPRB_EPI_DGELU_PRE = 6,      /* D(bf16) = acc * gelu'(aux), aux(bf16) = the PRE-activation saved by BIAS_GELU|SAVE_PRE */
   DPRB_EPI_COUNT = 7
 };
-/* OR-ed into `epilogue`: the named 16-bit operand holds IEEE fp16 instead of bf16 (tcgen05 kind::f16 takes either
- * format per operand).  The encoder keeps its residual stream - LayerNorm inputs and outputs - in fp16 (11 significand
+/* OR-ed into `epilogue`: the named 16-bit operand holds IEEE fp16 instead of bf16 (wgmma takes one
+ * format for both operands: give DPRB_GEMM_A_F16 and DPRB_GEMM_B_F16 together or not at all).  The encoder keeps its residual stream - LayerNorm inputs and outputs - in fp16 (11 significand
  * bits in the same 2 bytes): these are the tensors HF's autocast keeps in fp32 (modeling_bert.py:296-298, :354-356
  * run LayerNorm and the residual add outside the 16-bit region).  AUX / OUT apply to the BIAS and BIAS_RESIDUAL
  * epilogues. */
@@ -169,11 +169,11 @@ int dprb_score_ce_bwd(const float* q, const float* c, const float* logits, const
                       int C, int d, int q0, int nq, int c0, int nc, dprb_stream_t stream);
 
 /* The same operator on the tensor cores, in ONE pass (the form BASELINE.json's north_star names): similarity tile via
- * tcgen05.mma into TMEM, online row max / sum-exp / label pick straight from tcgen05.ld, loss accumulated by the last
+ * wgmma tiles staged in shared memory, online row max / sum-exp / label pick per row, loss accumulated by the last
  * tile of each row block; logits reach HBM only if `logits` is non-NULL.  fp32 fidelity comes from an exact 3-way bf16
  * split of q and c (six partial products per k-block, fp32 accumulate): logits agree with the fp32 product of
  * dpr_task.py:99 to ~1e-6 relative.  Backward RECOMPUTES the tiles of the rank-local row block and column block
- * (no stored logits) and runs dq = W_rows c, dc = W_cols^T q on the tcgen05 GEMM.
+ * (no stored logits) and runs dq = W_rows c, dc = W_cols^T q on the library's GEMM.
  *   nq / nc: the local row / column counts backward will ask for (sizes the workspace; -1 = all).
  *   workspace: caller-owned, 256-byte aligned, >= dprb_score_tc_workspace_bytes(...); it carries the operand splits
  *   from the forward call to the backward call of the same step.
@@ -192,7 +192,8 @@ int dprb_score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const i
  * (conf/task/optim/adamw.yaml via dpr_task.py:124) + clip_grad_norm_(2.0)
  * (conf/trainer/gpu_1_host.yaml:8) + the bf16 weight shadow refresh.
  *   dprb_sumsq: out[0] += sum g^2.
- *   dprb_adamw_step: coef = min(1, max_norm / (sqrt(*sumsq) * grad_div_inv... see DESIGN.md) applied to g.
+ *   dprb_adamw_step: coef = min(1, max_norm / (sqrt(*sumsq) * grad_scale) + 1e-6) multiplies grad_scale * g
+ *   before the moments are updated (optim.cu).
  * ------------------------------------------------------------------------------------------- */
 int dprb_sumsq_f32(const float* g, int64_t n, float* out, dprb_stream_t stream);
 int dprb_adamw_step(float* p, const float* g, float* m, float* v, void* shadow_bf16, int64_t n, float lr,
@@ -239,8 +240,8 @@ typedef struct {
                               * x1, the FFN pre-activation and the layer output, and REBUILD the attention output
                               * (one more attention forward) and gelu / gelu' (from the pre-activation) in backward:
                               * 22 KB instead of 32 KB per token and layer at RoBERTa-large, which is what lets
-                              * BASELINE config 4 (278 528 tokens x 24 layers per GPU) fit 180 GB without recomputing
-                              * the whole forward. */
+                              * RoBERTa-large at S = 256 train on an 80 GB H100 without recomputing the whole
+                              * forward. */
   float dropout_p;           /* hidden + attention-probability dropout (HFEncoder's `dropout`); 0 in eval mode */
   uint64_t dropout_seed;     /* per-forward seed; backward must be given the same value */
 } dprb_encoder_batch;
@@ -256,10 +257,10 @@ int dprb_encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b,
                      int layer_lo, int layer_hi, dprb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Brute-force retrieval (SURVEY.md section 8f row 3): replaces search_index() of
+ * Brute-force retrieval : replaces search_index() of
  * dpr_scale/run_retrieval_pytorch.py:141-176 -- einsum('ik,jk->ij') in fp16 followed by torch.topk over the
  * materialised [Q, N] score matrix -- with one fused pass: the corpus is streamed once per block of 128 queries
- * through tcgen05 and a running top-k is kept per query; no score matrix is written.
+ * through wgmma and a running top-k is kept per query; no score matrix is written.
  *   queries [Q, d], corpus [N, d]: row-major 16-bit (dtype 0 = fp16 as in build_index() :178-190, 1 = bf16),
  *   d % 8 == 0, 16-byte aligned, N < 2^31 - 256, 1 <= k <= min(N, 1024).
  *   out_scores [Q, k] fp32 (fp32-accumulated inner products, descending; ties towards the lower row id),

@@ -6,7 +6,7 @@
 The reference cannot travel to the GPU box, so the vectors are committed.  What runs here:
   * dpr_scale.models.hf_model.HFEncoder               (imported as is)
   * dpr_scale.task.dpr_task.DenseRetrieverTask        (imported as is, through stub `hydra` /
-    `pytorch_lightning` modules because neither library is installed: SURVEY.md §8c / App. A3-A4).
+    `pytorch_lightning` modules because neither library is installed).
     The stub LightningModule.all_gather reproduces PL 1.6.4 semantics: per tensor dist.all_gather ->
     torch.stack(dim=0) under no_grad; identity when not distributed.
 Cases:

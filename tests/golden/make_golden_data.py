@@ -7,7 +7,7 @@ written by this script, and stores every batch it produces.
   python tests/golden/make_golden_data.py     # writes tests/golden/data/{synth.jsonl,vocab.txt} and data_batches.npz
 
 hydra / pytorch_lightning / ujson are not installed: the reference modules are imported through stub modules
-(hydra.utils.instantiate, pytorch_lightning.LightningDataModule, ujson := json), SURVEY.md App. A9.
+(hydra.utils.instantiate, pytorch_lightning.LightningDataModule, ujson := json).
 """
 import json
 import os

@@ -4,10 +4,10 @@
   python tests/golden/make_golden_realdims.py          # writes tests/golden/realdims_<case>.npz  (~1 min, 6 GB RAM)
 
 Same machinery as make_golden.py (stub `hydra` / `pytorch_lightning`, the reference's own HFEncoder +
-DenseRetrieverTask.training_step).  The weights come from the seeded recipe of tests/realdims.py (BASELINE.md §5) and are
+DenseRetrieverTask.training_step).  The weights come from the seeded recipe of tests/realdims.py and are
 NOT stored - only their fp64 checksums, so the GPU test can prove it rebuilt the same weights.  Stored per case:
 query / context embeddings, logits, loss, the reference's own bf16-autocast loss and gradient deviation (the yardstick of
-SURVEY §8c), and a sample of the fp32 parameter gradients of (i) the contrastive step and (ii) a linear probe
+the GPU parity gates), and a sample of the fp32 parameter gradients of (i) the contrastive step and (ii) a linear probe
 L = sum(rep * P) on the context encoder (well conditioned: no cancellation between rows).
 """
 import os

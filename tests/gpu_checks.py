@@ -3,7 +3,7 @@
 Each check returns a dict of error figures and raises AssertionError when a stated tolerance is exceeded.
 Used by tests/test_ops_gpu.py (pytest -m gpu) and tools/gpu_diag.py (one subprocess per check).
 
-Tolerances (stated here, per the fp contract of BASELINE.json:north_star / SURVEY.md §8c):
+Tolerances (stated here, per the fp contract of BASELINE.json:north_star):
   * bf16-output kernels: |err| <= 2^-7 * max|ref| + small atol   (one bf16 rounding of the result plus fp32
     accumulation-order noise; inputs are the identical bf16-rounded values on both sides)
   * fp32-output kernels (scoring/CE, optimizer, wgrad): rel <= 1e-4 unless noted.
@@ -391,7 +391,7 @@ CHECKS = {
     "adamw": lambda: check_adamw(),
 }
 
-# tcgen05 attention (S <= 128) extra shapes: many problems (persistent loop, barrier phases), heads=12
+# attention (S <= 128) extra shapes: many problems, heads=12
 CHECKS["score_ce_8gpu_shape"] = lambda: check_score_ce(Q=1024, C=8192, d=768, inv_t=0.125, q0=256, nq=128, c0=2048,
                                                        nc=1024, seed=16)     # cfg 3: global 1024 x 8192 scores per rank
 CHECKS["score_ce_pair_mask"] = lambda: check_score_ce(Q=130, C=300, d=128, inv_t=1.0, q0=1, nq=129, c0=0, nc=300, seed=17, pair=True)
@@ -408,7 +408,7 @@ CHECKS["attn_tc_drop_s128"] = lambda: check_attention(4, 128, 2, True, seed=14, 
 CHECKS["attn_tc2_drop_s200"] = lambda: check_attention(3, 200, 2, True, seed=15, dropout=0.1)
 
 
-# ------------------------------------------------------------------ retrieval (SURVEY.md 8f row 3)
+# ------------------------------------------------------------------ retrieval
 def check_search(Q=100, N=5000, d=768, k=100, bf16=False, seed=20, mode="random", offset=0):
     """dprb_search_topk vs oracle/retrieval.py (restating run_retrieval_pytorch.py:141-176) on float64 scores.
 

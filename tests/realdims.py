@@ -1,9 +1,8 @@
-"""Deterministic recipes for the parity cases at BASELINE.json's REAL model dimensions (VERDICT r1, item 1).
+"""Deterministic recipes for the parity cases at BASELINE.json's REAL model dimensions.
 
 The weights are far too large to commit (BERT-base 0.44 GB, RoBERTa-large 1.4 GB), so both sides rebuild them from a
-seed with the recipe of BASELINE.md §5: `torch.manual_seed(0); BertModel(BertConfig())` (HF default init) for the query
-encoder, the same + 0.01 * randn (`manual_seed(1)`) for the context encoder; RoBERTa-large from the RobertaConfig of
-SURVEY.md §8c.  `tests/golden/make_golden_realdims.py` runs the UNMODIFIED reference on them here and commits
+seed: `torch.manual_seed(0); BertModel(BertConfig())` (HF default init) for the query
+encoder, the same + 0.01 * randn (`manual_seed(1)`) for the context encoder; RoBERTa-large from its published RobertaConfig.  `tests/golden/make_golden_realdims.py` runs the UNMODIFIED reference on them here and commits
 embeddings / logits / loss / a sample of gradients + fp64 checksums of the weights; the GPU tests rebuild the weights on
 the box, check the checksums (same torch + transformers => same RNG stream) and compare the CUDA path with the golden.
 """
@@ -56,7 +55,7 @@ def checksums(model):
 
 
 def tokens(gen, n, S, pad_id, kind):
-    """BASELINE.md §5 variant B: lengths ~ U{S/4..S}, ids ~ U{1000..29999}, [CLS] first, [SEP] last real position."""
+    """Benchmark inputs, variant B: lengths ~ U{S/4..S}, ids ~ U{1000..29999}, [CLS] first, [SEP] last real position."""
     lens = torch.randint(S // 4, S + 1, (n,), generator=gen)
     lens[0] = S
     ids = torch.randint(1000, 30000, (n, S), generator=gen)

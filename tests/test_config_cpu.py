@@ -165,10 +165,10 @@ def test_generation_scripts_wire_task_transform_and_datamodule(tmp_path, monkeyp
 
 
 def test_committed_bench_line_has_the_contract_keys():
-    """The bench line recorded in profiles/ (a real B200 run of `python bench.py`) carries every key of the bench
+    """The bench line recorded in profiles/ (a real H100 run of `python bench.py`) carries every key of the bench
     contract, with consistent values - guards the schema against accidental edits of bench.py's output dict."""
     import json
-    line = json.load(open(os.path.join(ROOT, "profiles", "r1_bench_default_line.json")))
+    line = json.load(open(os.path.join(ROOT, "profiles", "h100_bench_default_line.json")))
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
               "vs_baseline", "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
         assert k in line, k

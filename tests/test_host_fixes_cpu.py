@@ -1,4 +1,4 @@
-"""Host-side logic fixed in round 2 (ADVICE.md r1 / VERDICT.md r1), all runnable without a GPU:
+"""Host-side logic, all runnable without a GPU:
   * two live forwards of ONE encoder never share a save-for-backward workspace (shared_model=True aliasing);
   * a shared encoder hands its gradient slices to the all-reduce exactly once per step (last outstanding backward);
   * reference checkpoints written with transformers==3.4.0 (persistent `embeddings.position_ids`) load strictly;

@@ -66,7 +66,7 @@ def test_two_rank_global_negatives_match_reference():
 
 def _shared_worker(rank, world, port, ret):
     """shared_model=True (the reference's constructor default) on 2 ranks: ONE encoder back-propagates twice per step into
-    one gradient arena; the bucketed all-reduce must reduce every slice exactly once (ADVICE r1: it used to reduce twice).
+    one gradient arena; the bucketed all-reduce must reduce every slice exactly once.
     Reference semantics (dpr_task.py:163-195 + DDP): SUM over ranks of the per-rank gradients == gradient of the global
     loss, i.e. what ONE process computes on the concatenated batch."""
     sys.path.insert(0, ROOT)

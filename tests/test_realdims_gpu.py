@@ -1,4 +1,4 @@
-"""Parity of the ASSEMBLED CUDA path at BASELINE.json's real model dimensions (VERDICT r1, item 1) against goldens the
+"""Parity of the ASSEMBLED CUDA path at BASELINE.json's real model dimensions against goldens the
 unmodified reference produced (tests/golden/make_golden_realdims.py) and against the HF oracle run live on the host:
 
   * BERT-base H768 / L12 / A12 on config 1's shape (8 q + 16 ctx, S = 64, padded): embeddings, logits, loss, gradients
@@ -9,7 +9,7 @@ unmodified reference produced (tests/golden/make_golden_realdims.py) and against
   * `shared_model=True` (the reference's constructor default) with query and context passes of EQUAL shape;
   * the `projection_dim` head.
 
-Gates (SURVEY §8c, vs the fp32 reference): embeddings rel-L2 <= 1e-2; logits max-abs <= 1e-2 * max|logit|; the loss
+Gates (vs the fp32 reference): embeddings rel-L2 <= 1e-2; logits max-abs <= 1e-2 * max|logit|; the loss
 kernel within 2e-3 of the reference's cross-entropy formula evaluated on our own logits, and within max(5e-2, 2 x the
 measured max|dlogit|) of the reference's loss (cross-entropy is 2-Lipschitz in the logits); contrastive-step
 gradients no looser than 1.5x (global) / 3x (per tensor, floor 2.5e-2) the reference's own AMP deviation - the
@@ -80,7 +80,7 @@ def _check_step(name, loss_gate):
     assert abs(float(loss.detach()) - ce_own) <= 2e-3, (float(loss.detach()), ce_own)
     # (2) against the reference's loss.  Softmax cross-entropy is 2-Lipschitz in max|dlogit|, and the logits of these
     # random-init models are raw 768/1024-wide dot products at temperature 1 (|logit| up to several hundred), so the
-    # embedding gate above (1e-2 rel-L2) already implies a loss uncertainty well above SURVEY 8c's 5e-2: two
+    # embedding gate above (1e-2 rel-L2) already implies a loss uncertainty well above the 5e-2 loss gate: two
     # roundings of the same embedding accuracy (4.5e-3) gave 0.005 and 0.105 here.  Gate: 5e-2 OR the bound implied by
     # the measured logit error, whichever is larger.
     assert dloss <= max(loss_gate, 2.0 * dl), (float(loss.detach()), float(g["loss"]), "max|dlogit|", dl,
@@ -142,7 +142,7 @@ def _check_probe(task, g, name):
 
 
 def test_bert_base_cfg1_training_step_matches_reference():
-    # loss gate: SURVEY §8c's 5e-2 (the reference's own AMP deviates by 0.034 on this batch)
+    # loss gate: 5e-2 (the reference's own AMP deviates by 0.034 on this batch)
     task, g = _check_step("bert_base_cfg1", 5e-2)
     _check_probe(task, g, "bert_base_cfg1")
 

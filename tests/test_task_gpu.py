@@ -1,7 +1,7 @@
 """End-to-end parity of the CUDA path behind the reference's plugin surface (HFEncoder / DenseRetrieverTask)
 against golden vectors produced by the unmodified reference (tests/golden/make_golden.py).
 
-Tolerances (vs the fp32 reference; SURVEY.md §8c — the reference's own bf16 autocast deviates by emb rel-L2
+Tolerances (vs the fp32 reference; the reference's own bf16 autocast deviates by emb rel-L2
 5.5e-3, logits 3.5e-3 relative, loss 0.018):
   embeddings rel-L2 <= 1e-2 ; logits max-abs <= 1e-2 * max|logit| ; loss abs <= 5e-2.
 Gradients are checked twice:
@@ -223,7 +223,7 @@ def test_lean_activations_match_full_mode():
     torch.cuda.synchronize()
     assert torch.equal(rep0.detach(), rep1.detach())
     assert rel_l2(enc.grads, g0) <= 5e-3, rel_l2(enc.grads, g0)
-    # BASELINE config 4 (RoBERTa-large, 1024 contexts x 256 tokens per GPU): full mode cannot fit 180 GB, lean mode does
+    # BASELINE config 4 (RoBERTa-large, 1024 contexts x 256 tokens per GPU): lean mode needs under 0.72x the full mode's workspace
     w = _lib.EncoderWeights()
     w.hidden, w.inter, w.layers, w.heads = 1024, 4096, 24, 16
     full = _lib.load().dprb_encoder_workspace_bytes(ctypes.byref(w), 1024, 256, 1)

@@ -20,7 +20,7 @@ from dpr_scale_b200.models.hf_model import HFEncoder
 
 CFG = dict(vocab_size=30522, hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072,
            max_position_embeddings=512)
-FWD_FLOP_PER_TOKEN = 174_587_904          # SURVEY.md 8(d), BERT-base S=128
+FWD_FLOP_PER_TOKEN = 174_587_904          # BERT-base S=128: 2 x (4H^2 + 2HI) + 4SH per layer x 12
 
 
 def batches(B, S, n, seed=0):

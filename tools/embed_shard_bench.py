@@ -12,8 +12,7 @@ async D2H into the pinned ring -> rows appended to ``reps_{rank:04}.pkl`` by the
 :49.  The path shards with NO collective (utils/utils.py:83-91), so N GPUs are N independent streams.
 
 One JSON line (rank 0): passages/s of the whole job = total passages / max over ranks of the device-timed region
-(CUDA events around the loop + the final drain), per-rank numbers, the model-FLOP rate (22.35 GFLOP per passage forward,
-SURVEY 8d) against the measured dense bf16 peak, bytes moved per passage, the size of the files written, peak host RSS
+(CUDA events around the loop + the final drain), per-rank numbers, the model-FLOP rate (22.35 GFLOP per passage forward) against the measured dense bf16 peak, bytes moved per passage, the size of the files written, peak host RSS
 (the reference holds the shard twice in RAM: 2 x 4 x 768 x passages bytes).
 """
 import argparse
@@ -30,7 +29,7 @@ import torch.distributed as dist
 BERT_BASE = dict(model_type="bert", vocab_size=30522, hidden_size=768, num_hidden_layers=12, num_attention_heads=12,
                  intermediate_size=3072, max_position_embeddings=512, type_vocab_size=2, layer_norm_eps=1e-12,
                  pad_token_id=0)
-FWD_FLOP_PER_TOKEN = 174_587_904          # SURVEY.md 8(d), BERT-base S = 128
+FWD_FLOP_PER_TOKEN = 174_587_904          # BERT-base S = 128: 2 x (4H^2 + 2HI) + 4SH per layer x 12
 
 
 def main():
@@ -107,7 +106,7 @@ def main():
         p = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
         if os.path.exists(p):
             peaks = json.load(open(p))
-        peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
         slow_wall = max(float(s[1]) for s in allst)
         slow_dev = max(float(s[0]) for s in allst)
         total = args.passages_per_rank * world

@@ -51,9 +51,9 @@ gemm("gemm wgrad Wqkv", 3 * H, H, T, 1, 1, 4, f32=True)
 
 qkv = rnd(T, 3 * H)
 seed = ops.dropout_site_seed(7, 3, 1)
-ctx, lse = ops.attn_fwd(qkv, None, T // S, S, HEADS, True, 0.1, seed); idx.append("attention fwd (tcgen05, dropout 0.1)")
+ctx, lse = ops.attn_fwd(qkv, None, T // S, S, HEADS, True, 0.1, seed); idx.append("attention fwd (wgmma, dropout 0.1)")
 dctx = rnd(T, H)
-ops.attn_bwd(qkv, None, ctx, lse, dctx, T // S, S, HEADS, torch.zeros(3 * H, device=dev), 0.1, seed); idx.append("attention bwd (tcgen05, dropout 0.1)")
+ops.attn_bwd(qkv, None, ctx, lse, dctx, T // S, S, HEADS, torch.zeros(3 * H, device=dev), 0.1, seed); idx.append("attention bwd (wgmma, dropout 0.1)")
 
 z16 = rnd(T, H, dt=torch.float16, sc=2.0)
 gamma, beta = torch.ones(H, device=dev), torch.zeros(H, device=dev)
@@ -85,7 +85,7 @@ q, c = torch.randn(Q, d, device=dev, generator=g), torch.randn(C, d, device=dev,
 mask = torch.zeros(C, dtype=torch.uint8, device=dev)
 labels = torch.randint(0, C, (Q,), device=dev, generator=g)
 _, _, _, sctx = ops.score_fwd(q, c, mask, labels, 1.0, False, None, (128, 1024))
-idx += ["score: bf16 split of q", "score: bf16 split of c", "score fwd (tcgen05 tiles + online softmax + NLL), 1024 x 8192 x 768"]
+idx += ["score: bf16 split of q", "score: bf16 split of c", "score fwd (wgmma tiles + online softmax + NLL), 1024 x 8192 x 768"]
 ops.score_bwd(sctx, 1.0, 1.0, 256, 128, 2048, 1024)
 idx += ["score bwd: W tiles recomputed (local rows + local columns)"] + ["score bwd GEMM %d/6" % i for i in range(1, 7)]
 torch.cuda.synchronize()

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Input-pipeline microbenchmark (CPU side of SURVEY.md 8f row 4): seconds per training batch of cfg 2
+"""Input-pipeline microbenchmark (CPU side of the training step): seconds per training batch of cfg 2
 (128 queries, 1 + 7 contexts each, truncated to 128 tokens) from a synthetic DPR-format JSONL.
 
   python tools/pipeline_bench.py [rows] [batches]

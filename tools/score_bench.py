@@ -37,5 +37,5 @@ for Q, C, nq, nc in SHAPES:
     _, _, _, ctx = ops.score_fwd(q, c, mask, labels, 1.0, False, None, (nq, nc))
     f = timeit(lambda: ops.score_fwd(q, c, mask, labels, 1.0, False, None, (nq, nc)))
     b = timeit(lambda: ops.score_bwd(ctx, 1.0, 1.0, 0, nq, 0, nc))
-    print(f"Q={Q} C={C} tcgen05 single pass (bf16x3: 2-part split, 3 products): fwd {f:8.1f} us ({2.0*Q*C*d/f/1e6:6.2f} TFLOP/s of fp32-equivalent "
+    print(f"Q={Q} C={C} tensor-core single pass (bf16x3: 2-part split, 3 products): fwd {f:8.1f} us ({2.0*Q*C*d/f/1e6:6.2f} TFLOP/s of fp32-equivalent "
           f"work, {6.0*Q*C*d/f/1e6:6.1f} executed)   bwd(recompute W + 6 GEMMs) {b:8.1f} us", flush=True)

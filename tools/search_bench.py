@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Retrieval microbenchmark: dprb_search_topk (fused tcgen05 scoring + running top-k) vs the reference's GPU path
+"""Retrieval microbenchmark: dprb_search_topk (fused wgmma scoring + running top-k) vs the reference's GPU path
 (run_retrieval_pytorch.py:141-176: fp16 einsum into a [Q, N] matrix + torch.topk), same box, same operands.
 
   python tools/search_bench.py [N d Q k] ...      default: MS MARCO-sized and Wikipedia-sized indexes
@@ -20,7 +20,7 @@ def peak_gbs():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json"
     except Exception:
-        return 7700.0, "B200_PROFILING.md fallback"
+        return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def timeit(f, iters):
