@@ -1,10 +1,15 @@
 // bf16 GEMM for sm_90a: TMA -> 128B-swizzled smem ring (mbarrier pipeline) -> wgmma (fp32 accumulators in
-// registers) -> epilogue straight from the accumulator registers, with the fused bias / bias+GELU / bias+residual /
-// dGELU / fp32 split-K accumulate variants the encoder needs.
+// registers) -> epilogue with the fused bias / bias+GELU / bias+residual / dGELU / fp32 split-K accumulate variants
+// the encoder needs.
 //
-// One CTA computes a 128x128 tile: warpgroups 0 and 1 own rows [0, 64) and [64, 128) (wgmma m64n128k16), warp 8 is
-// the TMA producer.  3-stage ring of 32 KB, so two CTAs share an SM and one CTA's epilogue overlaps the other's
-// main loop.
+// Persistent: one CTA per SM walks the work units (output tile, K split) in a static stride order.  A unit is a
+// 128x256 tile: warpgroups 1 and 2 own rows [0, 64) and [64, 128) (wgmma m64n256k16, 128 fp32 accumulators per
+// thread), warpgroup 0 is the TMA producer (one thread issues, setmaxnreg hands its registers to the consumers).  The
+// 3-stage ring of 48 KB runs across unit boundaries, so the producer loads the next unit's first k-blocks while the
+// consumers run the current unit's epilogue.  16-bit outputs go through a per-warpgroup staging slab in shared memory:
+// the fragment-layout results are written there, then each warp stores whole 512-byte rows with 16-byte stores.  The
+// aux operand (residual, gelu'(pre) or pre-activation) comes in the same way.  fp32 outputs (split-K partial sums)
+// stay fragment-layout red.global.add.v2.f32 / st.global straight from the registers.
 //
 // Replaces, on the reference path, every torch.nn.Linear call inside HF BertLayer (QKV, attention output,
 // intermediate, output) and their autograd backward (dgrad / wgrad).
@@ -22,20 +27,28 @@ namespace dprb {
 namespace {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_N = 128;
+constexpr int BLOCK_N = 256;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
 constexpr int STAGES = 3;
-constexpr int TILE_BYTES = 128 * BLOCK_K * 2;         // 16 KB: one operand tile of a stage
-constexpr int STAGE_BYTES = 2 * TILE_BYTES;
+constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
+constexpr int B_TILE_BYTES = BLOCK_N * BLOCK_K * 2;   // 32 KB
+constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
 constexpr int NUM_CONSUMERS = 2;                      // warpgroups
-constexpr int NUM_THREADS = NUM_CONSUMERS * 128 + 32; // + one producer warp
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 128 /*barriers*/;
-static_assert(2 * SMEM_BYTES <= 227 * 1024, "two CTAs per SM must fit");
+constexpr int NUM_THREADS = (NUM_CONSUMERS + 1) * 128; // + the producer warpgroup
+constexpr int WG_ROWS = BLOCK_M / NUM_CONSUMERS;      // 64
+// Staging slab row pitch in 16-bit elements: +16 B per row puts the 8 rows a fragment store touches on distinct banks.
+constexpr int STG_LD = BLOCK_N + 8;
+constexpr int STG_BYTES = WG_ROWS * STG_LD * 2;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + NUM_CONSUMERS * STG_BYTES + 1024 /*align slack*/ + 128 /*barriers*/;
+static_assert(SMEM_BYTES <= 227 * 1024, "ring + staging must fit one CTA per SM");
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + NUM_CONSUMERS * 128 * CONSUMER_REGS <= 65536, "register file");
 
 struct GemmParams {
   int M, N, K;
   int num_m_blocks, num_n_blocks;
   int k_blocks_total, k_blocks_per_split, splits;
+  int units;           // num_m_blocks * num_n_blocks * splits
   int epilogue;
   void* D;
   long long ldd;
@@ -50,12 +63,31 @@ struct GemmParams {
   int save_pre;          // EPI_BIAS_GELU: out2 receives the pre-activation itself instead of gelu'(pre) (lean activations)
 };
 
+// Work unit u -> tile origin and k-block range.  Units of one split are consecutive and tiles run N-fastest, so the
+// ~one wave of units in flight at a time covers a band of A rows against all of B (the encoder's B is at most 4.7 MB,
+// so it stays in L2); the wgrad splits in flight share one K slice of both operands.
+struct Unit {
+  int m0, n0, kb0, kb1;
+};
+__device__ __forceinline__ Unit unit_at(const GemmParams& p, int u) {
+  const int tiles = p.num_m_blocks * p.num_n_blocks;
+  const int tile = u % tiles, split = u / tiles;
+  Unit w;
+  w.m0 = (tile / p.num_n_blocks) * BLOCK_M;
+  w.n0 = (tile % p.num_n_blocks) * BLOCK_N;
+  w.kb0 = split * p.k_blocks_per_split;
+  w.kb1 = min(w.kb0 + p.k_blocks_per_split, p.k_blocks_total);
+  return w;
+}
+
 __device__ __forceinline__ void red_add_v2_f32(float* p, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
+// barrier of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
 
 template <int A_MN, int B_MN, int F16>
-__device__ __forceinline__ void mma_kblock(float (&acc)[64], uint32_t sa, uint32_t sb, int accumulate_first) {
+__device__ __forceinline__ void mma_kblock(float (&acc)[128], uint32_t sa, uint32_t sb, int accumulate_first) {
   // K-major SW128: 8-row groups 1024 B apart; a k16 step is +32 B inside the swizzle row.
   // MN-major SW128: 64-element MN atoms BLOCK_K*128 B apart (LBO), 8-deep K groups 1024 B apart; a k16 step is
   // +16 rows of 128 B.
@@ -66,45 +98,161 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[64], uint32_t sa, uint32
 #pragma unroll
   for (int k = 0; k < BLOCK_K / 16; ++k) {
     const int accum = (k > 0 || accumulate_first) ? 1 : 0;
-    if (F16) wgmma_m64n128_ss_f16<A_MN, B_MN>(acc, da + k * A_KSTEP, db + k * B_KSTEP, accum);
-    else wgmma_m64n128_ss_bf16<A_MN, B_MN>(acc, da + k * A_KSTEP, db + k * B_KSTEP, accum);
+    if (F16) wgmma_m64n256_ss_f16<A_MN, B_MN>(acc, da + k * A_KSTEP, db + k * B_KSTEP, accum);
+    else wgmma_m64n256_ss_bf16<A_MN, B_MN>(acc, da + k * A_KSTEP, db + k * B_KSTEP, accum);
   }
 }
 
 __device__ __forceinline__ uint32_t pack_out(float a, float b, bool f16) { return f16 ? pack_f16x2(a, b) : pack_bf16x2(a, b); }
-__device__ __forceinline__ void store_pair(bf16* base, long long off, int col, int N, uint32_t v) {
-  if (col + 1 < N) {
-    *reinterpret_cast<uint32_t*>(base + off) = v;
-  } else if (col < N) {
-    reinterpret_cast<uint16_t*>(base)[off] = (uint16_t)(v & 0xFFFFu);
+
+// The warpgroup's 64 x 256 slab of 16-bit values as 64 * 32 chunks of 16 B; thread t moves chunks t + 128 j, so each
+// warp covers one 512-byte row per step.  Rows >= M and columns >= N are skipped (a chunk straddling N goes element by
+// element).  Global rows and columns are 16-byte aligned: the host requires ld % 8 == 0 and 16-byte aligned bases.
+__device__ __forceinline__ void slab_store(const uint8_t* stg, uint16_t* g, long long ld, int row0, int n0, int M, int N,
+                                           int t) {
+#pragma unroll 4
+  for (int j = 0; j < WG_ROWS * BLOCK_N / 8 / 128; ++j) {
+    const int idx = t + 128 * j, r = idx >> 5, col = n0 + (idx & 31) * 8;
+    if (row0 + r >= M || col >= N) continue;
+    const uint4 v = *reinterpret_cast<const uint4*>(stg + r * (STG_LD * 2) + (idx & 31) * 16);
+    uint16_t* dst = g + (long long)(row0 + r) * ld + col;
+    if (col + 8 <= N) {
+      *reinterpret_cast<uint4*>(dst) = v;
+    } else {
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (col + e < N) dst[e] = (uint16_t)(w[e >> 1] >> (16 * (e & 1)));
+    }
   }
 }
-__device__ __forceinline__ float2 load_pair(const bf16* base, long long off, int col, int N, bool f16) {
-  uint32_t u = 0;
-  if (col + 1 < N) u = *reinterpret_cast<const uint32_t*>(base + off);
-  else if (col < N) u = reinterpret_cast<const uint16_t*>(base)[off];
-  return unpack_16x2(u, f16);
+__device__ __forceinline__ void slab_load(uint8_t* stg, const uint16_t* g, long long ld, int row0, int n0, int M, int N,
+                                          int t) {
+#pragma unroll 4
+  for (int j = 0; j < WG_ROWS * BLOCK_N / 8 / 128; ++j) {
+    const int idx = t + 128 * j, r = idx >> 5, col = n0 + (idx & 31) * 8;
+    if (row0 + r >= M || col >= N) continue;
+    const uint16_t* src = g + (long long)(row0 + r) * ld + col;
+    uint4 v;
+    if (col + 8 <= N) {
+      v = __ldg(reinterpret_cast<const uint4*>(src));
+    } else {
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (col + e < N) w[e >> 1] |= (uint32_t)__ldg(src + e) << (16 * (e & 1));
+      v = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    *reinterpret_cast<uint4*>(stg + r * (STG_LD * 2) + (idx & 31) * 16) = v;
+  }
+}
+
+// fp32 output straight from the fragment registers: split-K partial sums (red.global.add) or a plain store + bias
+template <bool ATOMIC>
+__device__ __forceinline__ void epilogue_f32(const GemmParams& p, const float (&acc)[128], int row0, int n0, int lr, int q) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + lr + 8 * h;
+    if (row >= p.M) continue;
+    float* drow = reinterpret_cast<float*>(p.D) + (long long)row * p.ldd;
+#pragma unroll
+    for (int c = 0; c < 32; ++c) {
+      const int col = n0 + 8 * c + 2 * q;
+      const float x = acc[4 * c + 2 * h] * p.alpha, y = acc[4 * c + 2 * h + 1] * p.alpha;
+      if (ATOMIC) {
+        if (col + 1 < p.N) red_add_v2_f32(drow + col, x, y);
+        else if (col < p.N) atomicAdd(drow + col, x);
+      } else {
+        if (col < p.N) drow[col] = x + (p.bias != nullptr ? __ldg(p.bias + col) : 0.f);
+        if (col + 1 < p.N) drow[col + 1] = y + (p.bias != nullptr ? __ldg(p.bias + col + 1) : 0.f);
+      }
+    }
+  }
+}
+
+// 16-bit epilogues: the fragment-layout results go to the warpgroup's staging slab (which holds aux, if any, on entry).
+// One instantiation per (epilogue, dropout, column sums), picked once per tile: the fully unrolled loop of each stays
+// a short straight run of code, where one loop branching on all of them per element pair spans ~170 KB of SASS and
+// misses the instruction cache on every tile.  EPI_BIAS_GELU leaves out2's values in acc.
+template <int EP, bool DROP, bool COLSUM>
+__device__ __forceinline__ void epilogue16(const GemmParams& p, float (&acc)[128], uint8_t* stg, int row0, int n0, int lr,
+                                           int q, int lane) {
+  const bool out_f16 = p.out_f16 != 0, aux_f16 = p.aux_f16 != 0;
+#pragma unroll
+  for (int c = 0; c < 32; ++c) {
+    const int col = n0 + 8 * c + 2 * q;
+    float2 b = make_float2(0.f, 0.f);
+    if (p.bias != nullptr) {
+      if (col + 1 < p.N) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+      else if (col < p.N) b.x = __ldg(p.bias + col);
+    }
+    float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + lr + 8 * h;
+      uint32_t* sp = reinterpret_cast<uint32_t*>(stg + (lr + 8 * h) * (STG_LD * 2) + (8 * c + 2 * q) * 2);
+      float2 v = ffma2(make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]), make_float2(p.alpha, p.alpha), b);
+      if constexpr (EP == DPRB_EPI_BIAS_GELU) {
+        float2 g, d;
+        gelu_and_grad2(v, g, d);
+        if (p.save_pre) d = v;        // lean activations: keep pre, rebuild gelu / gelu' in backward
+        *sp = pack_bf16x2(g.x, g.y);
+        acc[4 * c + 2 * h] = d.x;
+        acc[4 * c + 2 * h + 1] = d.y;
+        continue;
+      }
+      if constexpr (DROP) {
+        float m0f, m1f;
+        p.drop.mul2((uint32_t)row, (uint32_t)col, m0f, m1f);
+        v.x *= m0f; v.y *= m1f;
+      }
+      if constexpr (EP == DPRB_EPI_BIAS_RESIDUAL) {
+        const float2 a = unpack_16x2(*sp, aux_f16);
+        v.x += a.x; v.y += a.y;
+      } else if constexpr (EP == DPRB_EPI_DGELU) {
+        const float2 a = unpack_bf16x2(*sp);   // aux holds gelu'(pre) written by the forward epilogue
+        v.x *= a.x; v.y *= a.y;
+      } else if constexpr (EP == DPRB_EPI_DGELU_PRE) {
+        float2 g, d;                           // aux holds the pre-activation: derivative rebuilt (same fitted function)
+        gelu_and_grad2(unpack_bf16x2(*sp), g, d);
+        v.x *= d.x; v.y *= d.y;
+      }
+      const uint32_t o = pack_out(v.x, v.y, out_f16);
+      *sp = o;
+      if (COLSUM && row < p.M && col < p.N) {   // bias gradient: sums of the bf16-rounded output
+        const float2 f = unpack_bf16x2(o);
+        cs0 += f.x;
+        if (col + 1 < p.N) cs1 += f.y;
+      }
+    }
+    if (COLSUM) {
+      // lanes with the same q hold the same columns: reduce over the 8 row groups of the warp
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) {
+        cs0 += __shfl_xor_sync(0xFFFFFFFFu, cs0, o);
+        cs1 += __shfl_xor_sync(0xFFFFFFFFu, cs1, o);
+      }
+      if (lane < 4) {
+        if (col < p.N) atomicAdd(p.colsum + col, cs0);
+        if (col + 1 < p.N) atomicAdd(p.colsum + col + 1, cs1);
+      }
+    }
+  }
 }
 
 template <int A_MN, int B_MN, int F16>
-__global__ void __launch_bounds__(NUM_THREADS, 2)
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B needs 1024-byte aligned tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES]
-  uint64_t* empty_bar = full_bar + STAGES;                                           // [STAGES]
+  uint8_t* staging = smem + STAGES * STAGE_BYTES;                                     // [NUM_CONSUMERS][STG_BYTES]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + NUM_CONSUMERS * STG_BYTES);   // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                                // [STAGES]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int tiles = p.num_m_blocks * p.num_n_blocks;
-  const int u = blockIdx.x;
-  const int tile = u % tiles, split = u / tiles;
-  const int m_blk = tile / p.num_n_blocks, n_blk = tile % p.num_n_blocks;
-  const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
-  const int kb0 = split * p.k_blocks_per_split;
-  const int kb1 = min(kb0 + p.k_blocks_per_split, p.k_blocks_total);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
@@ -117,159 +265,129 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
   __syncthreads();
 
-  if (warp == NUM_CONSUMERS * 4) {
+  if (warp < 4) {
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
-        uint8_t* sa = smem + stage * STAGE_BYTES;
-        uint8_t* sb = sa + TILE_BYTES;
-        if (A_MN == 0) {
-          tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, m0);
-        } else {
+      for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+        const Unit w = unit_at(p, u);
+        for (int kb = w.kb0; kb < w.kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
+          uint8_t* sa = smem + stage * STAGE_BYTES;
+          uint8_t* sb = sa + A_TILE_BYTES;
+          if (A_MN == 0) {
+            tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, w.m0);
+          } else {
 #pragma unroll
-          for (int i = 0; i < BLOCK_M / 64; ++i) tma_load_2d(sa + i * (BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, kb * BLOCK_K);
-        }
-        if (B_MN == 0) {
-          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, n0);
-        } else {
+            for (int i = 0; i < BLOCK_M / 64; ++i) tma_load_2d(sa + i * (BLOCK_K * 128), &tmap_a, &full_bar[stage], w.m0 + i * 64, kb * BLOCK_K);
+          }
+          if (B_MN == 0) {
+            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, w.n0);
+          } else {
 #pragma unroll
-          for (int i = 0; i < BLOCK_N / 64; ++i) tma_load_2d(sb + i * (BLOCK_K * 128), &tmap_b, &full_bar[stage], n0 + i * 64, kb * BLOCK_K);
+            for (int i = 0; i < BLOCK_N / 64; ++i) tma_load_2d(sb + i * (BLOCK_K * 128), &tmap_b, &full_bar[stage], w.n0 + i * 64, kb * BLOCK_K);
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
     return;
   }
 
   // ================================ consumer warpgroups ================================
-  const int wg = warp >> 2;
-  float acc[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-  {
-    int stage = 0, prev = -1;
-    uint32_t phase = 0;
-    // this warpgroup's 64 rows of the A tile: K-major +64 rows of 128 B, MN-major the second 64-wide MN atom
-    const uint32_t a_off = (uint32_t)wg * (A_MN ? BLOCK_K * 128 : 64 * 128);
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + a_off;
-      const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES + TILE_BYTES);
-      wgmma_fence();
-      mma_kblock<A_MN, B_MN, F16>(acc, sa, sb, kb > kb0);
-      wgmma_commit();
-      // keep one k-block of MMAs in flight; the one before it has retired and its stage can be refilled
-      wgmma_wait<1>();
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
+  const int wg = (warp >> 2) - 1;
+  const int t = threadIdx.x - 128 * (wg + 1);
+  uint8_t* stg = staging + wg * STG_BYTES;
+  // this warpgroup's 64 rows of the A tile: K-major +64 rows of 128 B, MN-major the second 64-wide MN atom
+  const uint32_t a_off = (uint32_t)wg * (A_MN ? BLOCK_K * 128 : 64 * 128);
+  // fragment coordinates: the thread holds slab rows lr (d[4c], d[4c+1]) and lr + 8 (d[4c+2], d[4c+3]) at columns
+  // 8c + 2q, +1
+  const int q = lane & 3;
+  const int lr = (warp & 3) * 16 + (lane >> 2);
+  const int ep = p.epilogue;
+  const bool has_aux = (ep == DPRB_EPI_BIAS_RESIDUAL || ep == DPRB_EPI_DGELU || ep == DPRB_EPI_DGELU_PRE);
+
+  float acc[128];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+    const Unit w = unit_at(p, u);
+    {
+      int prev = -1;
+      for (int kb = w.kb0; kb < w.kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + a_off;
+        const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES + A_TILE_BYTES);
+        wgmma_fence();
+        mma_kblock<A_MN, B_MN, F16>(acc, sa, sb, kb > w.kb0);
+        wgmma_commit();
+        // keep one k-block of MMAs in flight; the one before it has retired and its stage can be refilled
+        wgmma_wait<1>();
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      prev = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    if (prev >= 0) {
+      wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
     }
-  }
 
-  // ================================ epilogue from registers ================================
-  // thread holds rows r0 (d[4c], d[4c+1]) and r0 + 8 (d[4c+2], d[4c+3]) at columns n0 + 8c + 2q, +1
-  const int q = lane & 3;
-  const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int ep = p.epilogue;
-  const bool f32_out = (ep == DPRB_EPI_F32_ATOMIC_ADD || ep == DPRB_EPI_F32_STORE);
-  if (f32_out) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r0 + 8 * h;
-      if (row >= p.M) continue;
-      float* drow = reinterpret_cast<float*>(p.D) + (long long)row * p.ldd;
-#pragma unroll
-      for (int c = 0; c < 16; ++c) {
-        const int col = n0 + 8 * c + 2 * q;
-        const float x = acc[4 * c + 2 * h] * p.alpha, y = acc[4 * c + 2 * h + 1] * p.alpha;
-        if (ep == DPRB_EPI_F32_ATOMIC_ADD) {
-          if (col + 1 < p.N) red_add_v2_f32(drow + col, x, y);
-          else if (col < p.N) atomicAdd(drow + col, x);
+    // ================================ epilogue ================================
+    const int row0 = w.m0 + wg * WG_ROWS;   // first global row of this warpgroup's slab
+    switch (ep) {
+      case DPRB_EPI_F32_ATOMIC_ADD: epilogue_f32<true>(p, acc, row0, w.n0, lr, q); continue;
+      case DPRB_EPI_F32_STORE: epilogue_f32<false>(p, acc, row0, w.n0, lr, q); continue;
+      default: break;
+    }
+    wg_bar(wg);   // the previous unit's slab_store has read the slab
+    if (has_aux) {
+      slab_load(stg, reinterpret_cast<const uint16_t*>(p.aux), p.ld_aux, row0, w.n0, p.M, p.N, t);
+      wg_bar(wg);
+    }
+    const bool cs = p.colsum != nullptr, drop = p.drop.on();
+    switch (ep) {
+      case DPRB_EPI_BIAS:
+        if (cs) epilogue16<DPRB_EPI_BIAS, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
+        else epilogue16<DPRB_EPI_BIAS, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+        break;
+      case DPRB_EPI_BIAS_GELU: epilogue16<DPRB_EPI_BIAS_GELU, false, false>(p, acc, stg, row0, w.n0, lr, q, lane); break;
+      case DPRB_EPI_BIAS_RESIDUAL:
+        if (drop) {
+          if (cs) epilogue16<DPRB_EPI_BIAS_RESIDUAL, true, true>(p, acc, stg, row0, w.n0, lr, q, lane);
+          else epilogue16<DPRB_EPI_BIAS_RESIDUAL, true, false>(p, acc, stg, row0, w.n0, lr, q, lane);
         } else {
-          if (col < p.N) drow[col] = x + (p.bias != nullptr ? __ldg(p.bias + col) : 0.f);
-          if (col + 1 < p.N) drow[col + 1] = y + (p.bias != nullptr ? __ldg(p.bias + col + 1) : 0.f);
+          if (cs) epilogue16<DPRB_EPI_BIAS_RESIDUAL, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
+          else epilogue16<DPRB_EPI_BIAS_RESIDUAL, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
         }
-      }
+        break;
+      case DPRB_EPI_DGELU:
+        if (cs) epilogue16<DPRB_EPI_DGELU, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
+        else epilogue16<DPRB_EPI_DGELU, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+        break;
+      default:
+        if (cs) epilogue16<DPRB_EPI_DGELU_PRE, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
+        else epilogue16<DPRB_EPI_DGELU_PRE, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+        break;
     }
-    return;
-  }
-  const bool out_f16 = p.out_f16 != 0;
-  bf16* D = reinterpret_cast<bf16*>(p.D);
+    wg_bar(wg);
+    slab_store(stg, reinterpret_cast<uint16_t*>(p.D), p.ldd, row0, w.n0, p.M, p.N, t);
+    if (ep == DPRB_EPI_BIAS_GELU && p.out2 != nullptr) {
+      wg_bar(wg);
 #pragma unroll
-  for (int c = 0; c < 16; ++c) {
-    const int col = n0 + 8 * c + 2 * q;
-    float2 b = make_float2(0.f, 0.f);
-    if (p.bias != nullptr) {
-      if (col + 1 < p.N) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-      else if (col < p.N) b.x = __ldg(p.bias + col);
-    }
-    float cs0 = 0.f, cs1 = 0.f;
+      for (int c = 0; c < 32; ++c)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r0 + 8 * h;
-      const bool ok = row < p.M && col < p.N;
-      float2 v = ffma2(make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]), make_float2(p.alpha, p.alpha), b);
-      const long long off = (long long)row * p.ldd + col;
-      if (ep == DPRB_EPI_BIAS_GELU) {
-        float2 g, d;
-        gelu_and_grad2(v, g, d);
-        if (p.save_pre) d = v;        // lean activations: keep pre, rebuild gelu / gelu' in backward
-        if (ok) {
-          if (p.out2 != nullptr) store_pair(p.out2, off, col, p.N, pack_bf16x2(d.x, d.y));
-          store_pair(D, off, col, p.N, pack_bf16x2(g.x, g.y));
-        }
-        continue;
-      }
-      if (ep == DPRB_EPI_BIAS_RESIDUAL && p.drop.on()) {
-        float m0f, m1f;
-        p.drop.mul2((uint32_t)row, (uint32_t)col, m0f, m1f);
-        v.x *= m0f; v.y *= m1f;
-      }
-      if (ep == DPRB_EPI_BIAS_RESIDUAL || ep == DPRB_EPI_DGELU || ep == DPRB_EPI_DGELU_PRE) {
-        const float2 a = ok ? load_pair(p.aux, (long long)row * p.ld_aux + col, col, p.N, p.aux_f16 != 0) : make_float2(0.f, 0.f);
-        if (ep == DPRB_EPI_BIAS_RESIDUAL) {
-          v.x += a.x; v.y += a.y;
-        } else if (ep == DPRB_EPI_DGELU) {
-          v.x *= a.x; v.y *= a.y;       // aux holds gelu'(pre) written by the forward epilogue
-        } else {
-          float2 g, d;                  // aux holds the pre-activation: derivative rebuilt (same fitted function)
-          gelu_and_grad2(a, g, d);
-          v.x *= d.x; v.y *= d.y;
-        }
-      }
-      const uint32_t o = pack_out(v.x, v.y, out_f16);
-      if (ok) {
-        store_pair(D, off, col, p.N, o);
-        if (p.colsum != nullptr) {      // bias gradient: sums of the bf16-rounded output
-          const float2 f = unpack_bf16x2(o);
-          cs0 += f.x;
-          if (col + 1 < p.N) cs1 += f.y;
-        }
-      }
-    }
-    if (p.colsum != nullptr) {
-      // lanes with the same q hold the same columns: reduce over the 8 row groups of the warp
-#pragma unroll
-      for (int o = 4; o < 32; o <<= 1) {
-        cs0 += __shfl_xor_sync(0xFFFFFFFFu, cs0, o);
-        cs1 += __shfl_xor_sync(0xFFFFFFFFu, cs1, o);
-      }
-      if (lane < 4) {
-        if (col < p.N) atomicAdd(p.colsum + col, cs0);
-        if (col + 1 < p.N) atomicAdd(p.colsum + col + 1, cs1);
-      }
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<uint32_t*>(stg + (lr + 8 * h) * (STG_LD * 2) + (8 * c + 2 * q) * 2) =
+              pack_bf16x2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]);
+      wg_bar(wg);
+      slab_store(stg, reinterpret_cast<uint16_t*>(p.out2), p.ldd, row0, w.n0, p.M, p.N, t);
     }
   }
 }
@@ -325,13 +443,15 @@ struct GemmProfile {
 GemmProfile g_prof;
 
 int choose_splits(int tiles, int k_blocks, int sms) {
-  // minimise the makespan ceil(tiles*s/sms)/s over s, keeping >= 4 k-blocks per split
+  // One CTA per SM walks ceil(tiles*s/sms) units of ceil(k_blocks/s) k-blocks each; every unit also pays about 4
+  // k-blocks' worth for its fp32 atomic epilogue (a 128x256 tile = 128 KB of red.global.add), which keeps s from
+  // growing for a marginally better fit.  Minimise that makespan, keeping >= 4 k-blocks per split.
   int best = 1;
   double best_cost = 1e30;
   for (int s = 1; s <= 32; ++s) {
     if (k_blocks / s < 4 && s > 1) break;
-    int waves = (tiles * s + sms - 1) / sms;
-    double cost = (double)waves / s + 0.002 * s;  // small penalty for extra atomic traffic
+    const int rounds = (tiles * s + sms - 1) / sms;
+    const double cost = (double)rounds * ((k_blocks + s - 1) / s + 4);
     if (cost < best_cost - 1e-9) { best_cost = cost; best = s; }
   }
   return best;
@@ -360,7 +480,8 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   DPRB_REQUIRE(!f32_out || (ldd % 4 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0),
                "gemm: fp32 output must be 16-byte aligned with ldd %% 4 == 0 (ldd=%lld)", ldd);
   if (epilogue == DPRB_EPI_BIAS_RESIDUAL || epilogue == DPRB_EPI_DGELU || epilogue == DPRB_EPI_DGELU_PRE)
-    DPRB_REQUIRE(aux != nullptr && ld_aux % 8 == 0, "gemm: epilogue %d needs aux with ld %% 8 == 0", epilogue);
+    DPRB_REQUIRE(aux != nullptr && ld_aux % 8 == 0 && (reinterpret_cast<uintptr_t>(aux) & 15) == 0,
+                 "gemm: epilogue %d needs a 16-byte aligned aux with ld %% 8 == 0", epilogue);
   if (bias != nullptr) DPRB_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "gemm: bias not 16B aligned");
 
   DPRB_REQUIRE(colsum == nullptr || (!f32_out && epilogue != DPRB_EPI_BIAS_GELU),
@@ -381,7 +502,7 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   const int sms = num_sms();
   const int tiles = p.num_m_blocks * p.num_n_blocks;
   if (epilogue != DPRB_EPI_F32_ATOMIC_ADD) splits = 1;
-  else if (splits <= 0) splits = choose_splits(tiles, p.k_blocks_total, 2 * sms);   // two CTAs per SM
+  else if (splits <= 0) splits = choose_splits(tiles, p.k_blocks_total, sms);
   if (splits > p.k_blocks_total) splits = p.k_blocks_total;
   p.k_blocks_per_split = (p.k_blocks_total + splits - 1) / splits;
   p.splits = (p.k_blocks_total + p.k_blocks_per_split - 1) / p.k_blocks_per_split;
@@ -395,7 +516,8 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   if (epilogue == DPRB_EPI_BIAS_GELU && out2 != nullptr)
     DPRB_REQUIRE((reinterpret_cast<uintptr_t>(out2) & 15) == 0, "gemm: out2 not 16-byte aligned");
 
-  const int grid = tiles * p.splits;
+  p.units = tiles * p.splits;
+  const int grid = p.units < sms ? p.units : sms;   // persistent: one CTA per SM
   static bool attr_set = false;
   if (!attr_set) {
 #define DPRB_SET_ATTR(...) DPRB_CHECK_CUDA(cudaFuncSetAttribute(__VA_ARGS__, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));

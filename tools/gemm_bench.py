@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""Time the encoder's GEMM shapes/epilogues in isolation with CUDA events (inputs >> L2 each).
+"""Time the encoder's GEMM shapes/epilogues in isolation with CUDA events (inputs >> L2 each), each next to cuBLAS
+(torch.matmul on the same bf16 operands into a bf16 output, no epilogue) as an in-call yardstick.
   python tools/gemm_bench.py [T]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -23,6 +24,17 @@ def run(name, M, N, K, a_mn, b_mn, epi, aux=False, out2=False, colsum=False, f32
     lda = M if a_mn else K
     ldb = N if b_mn else K
     f = lambda: ops.gemm(A, B, D, M, N, K, lda, ldb, N, a_mn, b_mn, epi, bias, ax, N if aux else 0, o2, 1.0, 0 if f32 else 1, cs)
+    Am = A.T if a_mn else A          # [M, K] views of the same storage
+    Bm = B if b_mn else B.T          # [K, N]
+    C = torch.empty(M, N, device=dev, dtype=bf)
+    ms = timed(f, iters)
+    ms_cublas = timed(lambda: torch.matmul(Am, Bm, out=C), iters)
+    tf = lambda t: 2.0 * M * N * K / t / 1e9
+    print(f"{name:34s} M={M:7d} N={N:5d} K={K:7d}  {ms*1e3:9.1f} us  {tf(ms):8.1f} TF/s   cuBLAS {ms_cublas*1e3:9.1f} us "
+          f"{tf(ms_cublas):8.1f} TF/s", flush=True)
+
+
+def timed(f, iters):
     for _ in range(2):
         f()
     torch.cuda.synchronize()
@@ -32,8 +44,7 @@ def run(name, M, N, K, a_mn, b_mn, epi, aux=False, out2=False, colsum=False, f32
         f()
     e1.record()
     torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / iters
-    print(f"{name:34s} M={M:7d} N={N:5d} K={K:7d}  {ms*1e3:9.1f} us  {2.0*M*N*K/ms/1e9:8.1f} TF/s", flush=True)
+    return e0.elapsed_time(e1) / iters
 
 
 run("fwd qkv bias", T, 3 * H, H, 0, 0, 0)
