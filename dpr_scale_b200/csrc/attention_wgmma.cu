@@ -14,7 +14,7 @@
 // load, so only stores need row predicates.
 //
 // Replaces BertSelfAttention.forward's scaled_dot_product_attention and its autograd backward.
-#include "common.cuh"
+#include "attention.cuh"
 #include "dprb_internal.h"
 
 namespace dprb {
@@ -24,27 +24,11 @@ constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
 
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-
-// K-major operand: [rows][64] bf16, one swizzle atom wide, 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t desc_k(const void* p) { return make_wgmma_desc_sw128(smem_u32(p), 16, 1024); }
-// MN-major operand read from [K rows][64 MN] (a single 64-wide MN atom)
-__device__ __forceinline__ uint64_t desc_mn(const void* p) { return make_wgmma_desc_sw128(smem_u32(p), 16, 1024); }
-// descriptor steps of one k16 slice (16-byte units): K-major +32 B, MN-major +16 rows of 128 B
-constexpr uint64_t KSTEP_K = 2, KSTEP_MN = 128;
-
 template <int N>
 __device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, int acc) {
   if constexpr (N == 64) wgmma_m64n64_ss_bf16<0, 0>(d, a, b, acc);
   else if constexpr (N == 128) wgmma_m64n128_ss_bf16<0, 0>(d, a, b, acc);
   else wgmma_m64n256_ss_bf16<0, 0>(d, a, b, acc);
-}
-
-// keep multipliers of element (r, c) for a single column c (the pair hash covers columns c & ~1 and c | 1)
-__device__ __forceinline__ float drop_one(const Drop& d, uint32_t r, uint32_t c) {
-  float m0, m1;
-  d.mul2(r, c & ~1u, m0, m1);
-  return (c & 1u) ? m1 : m0;
 }
 
 // ------------------------------------------------------------------------------------------ forward
@@ -356,7 +340,10 @@ attn_bwd_wg_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   }
 }
 
+}  // namespace
+
 // ------------------------------------------------------------------------------------------ host
+namespace {
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -372,8 +359,8 @@ EncodeTiledFn encode_fn() {
   }
   return fn;
 }
+}  // namespace
 
-// bf16 [nseq, S, cols] (row stride `cols` elements), box = [1, box_rows, 64 cols], 128B swizzle
 int make_tmap3(CUtensorMap* out, const void* base, int nseq, int S, long long cols, int box_rows) {
   static thread_local bool ctx_bound = false;   // driver entry point: needs a current context on THIS thread
   if (!ctx_bound) {
@@ -393,6 +380,8 @@ int make_tmap3(CUtensorMap* out, const void* base, int nseq, int S, long long co
   DPRB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(3d) failed with CUresult %d", (int)r);
   return 0;
 }
+
+namespace {
 
 template <int NK>
 int fwd_launch(const CUtensorMap& tq, const CUtensorMap& tkv, const int32_t* attn_mask, void* ctx, float* lse, int nseq,

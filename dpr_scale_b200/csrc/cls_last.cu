@@ -4,7 +4,8 @@
 // tokens are still needed.  HuggingFace computes (and back-propagates) all S rows and throws S-1 of them away.
 //
 // Kernels here: single-query attention forward / backward (one warp per (sequence, head), exact fp32 softmax over
-// <= 256 keys) and the scatter of the CLS-row residual gradient.  The GEMMs / LayerNorms of the pruned layer are the
+// <= 512 keys: MAXK keys per lane, 8 for S <= 256 and 16 for 256 < S <= 512) and the scatter of the CLS-row residual
+// gradient.  The GEMMs / LayerNorms of the pruned layer are the
 // regular kernels run on nseq rows.
 //
 // Same arithmetic as BertSelfAttention (site-packages/transformers/models/bert/modeling_bert.py:168-207) restricted
@@ -14,8 +15,6 @@
 
 namespace dprb {
 namespace {
-
-constexpr int MAXK = 8;  // keys per lane: S <= 256
 
 __device__ __forceinline__ void load_row64(const bf16* p, float (&v)[64]) {
 #pragma unroll
@@ -53,7 +52,10 @@ __device__ __forceinline__ float drop_mul1(const Drop& d, uint32_t r, uint32_t c
 }
 
 // ctx_cls[seq, h*64 + d] = sum_j softmax_j(q_0 . k_j / 8 + mask_j) v_j[d];  probs[(seq*heads+h)*S + j] saved (fp32).
-__global__ void __launch_bounds__(256)
+// MAXK: keys per lane (S <= 32 * MAXK).  MAXK = 16 asks for one CTA per SM so that its 16-key rows fit in registers
+// without spilling; MAXK = 8 keeps the compiler's default (a minimum of 0 blocks is no constraint).
+template <int MAXK>
+__global__ void __launch_bounds__(256, MAXK == 8 ? 0 : 1)
 attn_cls_fwd_kernel(const bf16* __restrict__ qkv, const int32_t* __restrict__ attn_mask, bf16* __restrict__ ctx_cls,
                     float* __restrict__ probs, int nseq, int S, int heads, Drop drop) {
   const int lane = threadIdx.x & 31;
@@ -109,7 +111,8 @@ attn_cls_fwd_kernel(const bf16* __restrict__ qkv, const int32_t* __restrict__ at
 }
 
 // Backward of the single-query attention: writes the FULL dqkv [T, 3H] (dQ: row 0 only, zeros elsewhere).
-__global__ void __launch_bounds__(256)
+template <int MAXK>
+__global__ void __launch_bounds__(256, MAXK == 8 ? 0 : 1)
 attn_cls_bwd_kernel(const bf16* __restrict__ qkv, const float* __restrict__ probs, const bf16* __restrict__ dctx_cls,
                     bf16* __restrict__ dqkv, int nseq, int S, int heads, Drop drop) {
   const int lane = threadIdx.x & 31;
@@ -192,22 +195,28 @@ __global__ void add_rows_kernel(bf16* __restrict__ dst, const bf16* __restrict__
 
 int attn_cls_fwd(const void* qkv, const int32_t* attn_mask, void* ctx_cls, float* probs, int nseq, int S, int heads,
                  float dropout_p, unsigned long long site_seed, cudaStream_t stream) {
-  DPRB_REQUIRE(S >= 1 && S <= 32 * MAXK, "attn_cls_fwd: sequence length %d unsupported", S);
+  DPRB_REQUIRE(S >= 1 && S <= 512, "attn_cls_fwd: sequence length %d unsupported (1..512)", S);
   if (nseq == 0) return 0;
   const Drop drop = drop_from_site(dropout_p, site_seed);
   const int nprob = nseq * heads;
-  attn_cls_fwd_kernel<<<(nprob + 7) / 8, 256, 0, stream>>>((const bf16*)qkv, attn_mask, (bf16*)ctx_cls, probs, nseq, S, heads, drop);
+  if (S <= 256)
+    attn_cls_fwd_kernel<8><<<(nprob + 7) / 8, 256, 0, stream>>>((const bf16*)qkv, attn_mask, (bf16*)ctx_cls, probs, nseq, S, heads, drop);
+  else
+    attn_cls_fwd_kernel<16><<<(nprob + 7) / 8, 256, 0, stream>>>((const bf16*)qkv, attn_mask, (bf16*)ctx_cls, probs, nseq, S, heads, drop);
   DPRB_LAUNCH_CHECK();
   return 0;
 }
 
 int attn_cls_bwd(const void* qkv, const float* probs, const void* dctx_cls, void* dqkv, int nseq, int S, int heads,
                  float dropout_p, unsigned long long site_seed, cudaStream_t stream) {
-  DPRB_REQUIRE(S >= 1 && S <= 32 * MAXK, "attn_cls_bwd: sequence length %d unsupported", S);
+  DPRB_REQUIRE(S >= 1 && S <= 512, "attn_cls_bwd: sequence length %d unsupported (1..512)", S);
   if (nseq == 0) return 0;
   const Drop drop = drop_from_site(dropout_p, site_seed);
   const int nprob = nseq * heads;
-  attn_cls_bwd_kernel<<<(nprob + 7) / 8, 256, 0, stream>>>((const bf16*)qkv, probs, (const bf16*)dctx_cls, (bf16*)dqkv, nseq, S, heads, drop);
+  if (S <= 256)
+    attn_cls_bwd_kernel<8><<<(nprob + 7) / 8, 256, 0, stream>>>((const bf16*)qkv, probs, (const bf16*)dctx_cls, (bf16*)dqkv, nseq, S, heads, drop);
+  else
+    attn_cls_bwd_kernel<16><<<(nprob + 7) / 8, 256, 0, stream>>>((const bf16*)qkv, probs, (const bf16*)dctx_cls, (bf16*)dqkv, nseq, S, heads, drop);
   DPRB_LAUNCH_CHECK();
   return 0;
 }

@@ -45,6 +45,7 @@ int plan(const dprb_encoder_weights* w, int nseq, int S, int save, void* base, W
   DPRB_REQUIRE(w->layers >= 1 && w->layers <= 64, "encoder: layers=%d unsupported", w->layers);
   DPRB_REQUIRE(w->hidden % 8 == 0 && w->inter % 8 == 0 && w->hidden <= 1024, "encoder: H=%d I=%d unsupported", w->hidden, w->inter);
   DPRB_REQUIRE(w->heads * 64 == w->hidden, "encoder: head_dim must be 64 (H=%d heads=%d)", w->hidden, w->heads);
+  DPRB_REQUIRE(S <= 512, "encoder: sequence length %d unsupported (at most 512)", S);
   const long long T = (long long)nseq * S, H = w->hidden, I = w->inter;
   Carve c(base);
   ws->rA = (bf16*)c.take(T * H * 2);
@@ -138,6 +139,8 @@ long long encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S
 int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, cudaStream_t stream) {
   Workspace ws;
   TRY(plan(w, b->nseq, b->S, b->save_for_backward, b->workspace, &ws));
+  // position ids index a table of max_pos rows (RoBERTa's pad-derived ids need max_pos >= S + pad + 1: checked by the caller)
+  DPRB_REQUIRE(b->S <= w->max_pos, "encoder_fwd: sequence length %d exceeds the position table (max_pos %d)", b->S, w->max_pos);
   DPRB_REQUIRE(b->workspace != nullptr && b->workspace_bytes >= ws.bytes, "encoder_fwd: workspace too small (%lld < %lld)",
                (long long)b->workspace_bytes, ws.bytes);
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(b->workspace) & 255) == 0, "encoder_fwd: workspace must be 256-byte aligned");

@@ -502,6 +502,16 @@ class HFEncoder(nn.Module):
         dev = self.master.device
         ids = ids.to(dev, torch.int64).contiguous()
         N, S = ids.shape
+        # position ids must index the position table (HF raises an IndexError there); RoBERTa's are pad-derived and
+        # reach S + pad_token_id.  The attention kernels stop at 512 tokens.
+        max_pos = self.config["max_position_embeddings"]
+        roberta = self.config["model_type"] in ("roberta", "xlm-roberta")
+        limit = max_pos - self.config["pad_token_id"] - 1 if roberta else max_pos
+        if S > limit:
+            raise ValueError(f"sequence length {S} needs position ids beyond max_position_embeddings={max_pos} "
+                             f"(longest supported: {limit})")
+        if S > 512:
+            raise ValueError(f"sequence length {S} unsupported: the dprb kernels take at most 512 tokens")
         tt = tokens.get("token_type_ids") if hasattr(tokens, "get") else None
         tt = torch.zeros_like(ids) if tt is None else tt.to(dev, torch.int64).contiguous()
         am = tokens.get("attention_mask") if hasattr(tokens, "get") else None

@@ -134,13 +134,15 @@ int dprb_gelu_from_pre(const void* pre_bf16, void* out_bf16, int64_t n, dprb_str
 int dprb_colsum_bf16(const void* x_bf16, int64_t ld, float* out, int T, int N, dprb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Self-attention core for head_dim 64, S <= 256.  Replaces BertSelfAttention.forward's
+ * Self-attention core for head_dim 64, S <= 512.  Replaces BertSelfAttention.forward's
  * scaled_dot_product_attention (modeling_bert.py:168-207, integrations/sdpa_attention.py:92-101):
  *   ctx = softmax(Q K^T / 8 + key_mask) V      per (sequence, head).
  * qkv: bf16 [nseq*S, 3H] = [Q | K | V] column blocks, head h at columns h*64.
  * attn_mask: int32 [nseq, S], 1 = real token, 0 = padding (HF attention_mask); may be NULL.
  * lse: fp32 [nseq, heads, S] natural-log row log-sum-exp, written by fwd (may be NULL for
  *      forward-only use) and consumed by bwd together with the forward output ctx.
+ * Kernels: S <= 256 keeps every key of a row in one block; 256 < S <= 512 streams 128-key blocks with an online
+ * softmax, and its backward (one dK/dV and one dQ kernel, deterministic) takes D = rowsum(dctx * ctx) from ctx.
  * ------------------------------------------------------------------------------------------- */
 int dprb_attn_fwd(const void* qkv_bf16, const int32_t* attn_mask, void* ctx_bf16, float* lse, int nseq, int S,
                   int heads, float dropout_p, uint64_t dropout_site_seed, dprb_stream_t stream);
@@ -247,7 +249,9 @@ typedef struct {
 } dprb_encoder_batch;
 
 int64_t dprb_encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S, int save_for_backward);
-/* pooled fp32 [nseq, hidden] = last-layer hidden state of token 0 of each sequence. */
+/* pooled fp32 [nseq, hidden] = last-layer hidden state of token 0 of each sequence.
+ * Requires S <= 512 and S <= max_pos; every pos_ids entry must be < max_pos (RoBERTa's pad-derived ids reach
+ * S + pad_token_id, so there max_pos >= S + pad_token_id + 1). */
 int dprb_encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled,
                      dprb_stream_t stream);
 /* Accumulates parameter gradients into w->grads given dpooled fp32 [nseq, hidden].
