@@ -20,17 +20,6 @@ void set_last_error(const char* fmt, ...) {
 static std::atomic<long long> g_launches{0};
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
-int num_sms() {
-  static int cached = 0;
-  if (cached == 0) {
-    int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return -1;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
-    cached = n;
-  }
-  return cached;
-}
-
 }  // namespace dprb
 
 using namespace dprb;

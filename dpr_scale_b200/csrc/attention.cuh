@@ -8,21 +8,12 @@ constexpr float ATTN_SCALE_LOG2 = 0.125f * 1.4426950408889634f;   // 1/sqrt(64) 
 constexpr float ATTN_LOG2E = 1.4426950408889634f;
 constexpr float ATTN_LN2 = 0.6931471805599453f;
 
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-
 // K-major operand: [rows][64] bf16, one swizzle atom wide, 8-row groups 1024 B apart
 __device__ __forceinline__ uint64_t desc_k(const void* p) { return make_wgmma_desc_sw128(smem_u32(p), 16, 1024); }
 // MN-major operand read from [K rows][64 MN] (a single 64-wide MN atom)
 __device__ __forceinline__ uint64_t desc_mn(const void* p) { return make_wgmma_desc_sw128(smem_u32(p), 16, 1024); }
 // descriptor steps of one k16 slice (16-byte units): K-major +32 B, MN-major +16 rows of 128 B
 constexpr uint64_t KSTEP_K = 2, KSTEP_MN = 128;
-
-// keep multipliers of element (r, c) for a single column c (the pair hash covers columns c & ~1 and c | 1)
-__device__ __forceinline__ float drop_one(const Drop& d, uint32_t r, uint32_t c) {
-  float m0, m1;
-  d.mul2(r, c & ~1u, m0, m1);
-  return (c & 1u) ? m1 : m0;
-}
 
 // bf16 [nseq, S, cols] (row stride `cols` elements), box = [1, box_rows, 64 cols], 128B swizzle; rows >= S of a
 // sequence are zero-filled on load

@@ -40,10 +40,6 @@ static_assert(fwd_long_smem() <= 227 * 1024, "long attention forward: shared mem
 static_assert(dkdv_long_smem() <= 227 * 1024, "long attention dK/dV: shared memory budget exceeded");
 static_assert(dq_long_smem() <= 227 * 1024, "long attention dQ: shared memory budget exceeded");
 
-__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
-  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
-}
-
 // D_i = rowsum(dO_i * ctx_i) in fp32 and lse_i * log2(e) for rows r0 .. r0 + n - 1 of one problem (n a multiple of
 // 32; rows >= S get D = 0, lse2 = +inf so that P = 0).  Eight threads per row, 16-byte loads; 256 threads.
 __device__ __forceinline__ void rows_d_lse(const bf16* __restrict__ dctx, const bf16* __restrict__ ctx,

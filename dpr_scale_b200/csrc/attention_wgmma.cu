@@ -20,10 +20,6 @@
 namespace dprb {
 namespace {
 
-constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
-constexpr float LOG2E = 1.4426950408889634f;
-constexpr float LN2 = 0.6931471805599453f;
-
 template <int N>
 __device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, int acc) {
   if constexpr (N == 64) wgmma_m64n64_ss_bf16<0, 0>(d, a, b, acc);
@@ -41,7 +37,7 @@ attn_fwd_wg_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
                    const int32_t* __restrict__ attn_mask, bf16* __restrict__ ctx, float* __restrict__ lse_out, int S,
                    int heads, Drop drop) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   uint8_t* sQ = smem;                       // [64][64]
   uint8_t* sK = sQ + 64 * 128;              // [NK][64]
   uint8_t* sV = sK + NK * 128;              // [NK][64]
@@ -90,8 +86,8 @@ attn_fwd_wg_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
     for (int h2 = 0; h2 < 2; ++h2) {
       float& x = s[4 * c + 2 * h2];
       float& y = s[4 * c + 2 * h2 + 1];
-      x = fmaf(x, SCALE_LOG2, mk.x);
-      y = fmaf(y, SCALE_LOG2, mk.y);
+      x = fmaf(x, ATTN_SCALE_LOG2, mk.x);
+      y = fmaf(y, ATTN_SCALE_LOG2, mk.y);
       m[h2] = fmaxf(m[h2], fmaxf(x, y));
     }
   }
@@ -140,7 +136,7 @@ attn_fwd_wg_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   for (int h2 = 0; h2 < 2; ++h2) {
     const int row = qb * 64 + lrow + 8 * h2;
     if (row >= S) continue;
-    if (lse_out != nullptr && q4 == 0) lse_out[(long long)prob * S + row] = m[h2] * LN2 + __logf(l[h2]);
+    if (lse_out != nullptr && q4 == 0) lse_out[(long long)prob * S + row] = m[h2] * ATTN_LN2 + __logf(l[h2]);
     const float inv = l[h2] > 0.f ? 1.f / l[h2] : 0.f;
     bf16* dst = ctx + ((long long)seq * S + row) * H + h * 64;
 #pragma unroll
@@ -161,7 +157,7 @@ attn_bwd_wg_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
                    const int32_t* __restrict__ attn_mask, const float* __restrict__ lse_in, bf16* __restrict__ dqkv, int S,
                    int heads, Drop drop) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   uint8_t* sQ = smem;
   uint8_t* sdO = sQ + NK * 128;
   uint8_t* sK = sdO + NK * 128;
@@ -195,7 +191,7 @@ attn_bwd_wg_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   for (int j = tid; j < NK; j += 256) {
     const bool keep = j < S && (attn_mask == nullptr || attn_mask[(long long)seq * S + j] != 0);
     sMask[j] = keep ? 0.f : -INFINITY;
-    sLse[j] = j < S ? lse_in[(long long)prob * S + j] * LOG2E : INFINITY;   // rows beyond S: P = 0
+    sLse[j] = j < S ? lse_in[(long long)prob * S + j] * ATTN_LOG2E : INFINITY;   // rows beyond S: P = 0
     sD[j] = 0.f;
   }
   __syncthreads();
@@ -224,8 +220,8 @@ attn_bwd_wg_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
 #pragma unroll
         for (int h2 = 0; h2 < 2; ++h2) {
           const int i = 4 * c + 2 * h2;
-          float px = ex2_approx(fmaf(sc[i], SCALE_LOG2, mk.x) - ls[h2]);
-          float py = ex2_approx(fmaf(sc[i + 1], SCALE_LOG2, mk.y) - ls[h2]);
+          float px = ex2_approx(fmaf(sc[i], ATTN_SCALE_LOG2, mk.x) - ls[h2]);
+          float py = ex2_approx(fmaf(sc[i + 1], ATTN_SCALE_LOG2, mk.y) - ls[h2]);
           if (DROP) {
             float m0, m1;
             drop.mul2((uint32_t)(prob * S + qb * 64 + lrow + 8 * h2), (uint32_t)kcol, m0, m1);
@@ -268,8 +264,8 @@ attn_bwd_wg_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
 #pragma unroll
         for (int h2 = 0; h2 < 2; ++h2) {
           const int i = 4 * c + 2 * h2;
-          const float px = ex2_approx(fmaf(st[i], SCALE_LOG2, mk[h2]) - ls.x);
-          const float py = ex2_approx(fmaf(st[i + 1], SCALE_LOG2, mk[h2]) - ls.y);
+          const float px = ex2_approx(fmaf(st[i], ATTN_SCALE_LOG2, mk[h2]) - ls.x);
+          const float py = ex2_approx(fmaf(st[i + 1], ATTN_SCALE_LOG2, mk[h2]) - ls.y);
           float mx = 1.f, my = 1.f;
           if (DROP) {
             const uint32_t kr = (uint32_t)(kb * 64 + lrow + 8 * h2);
@@ -343,42 +339,13 @@ attn_bwd_wg_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
 }  // namespace
 
 // ------------------------------------------------------------------------------------------ host
-namespace {
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-}  // namespace
-
 int make_tmap3(CUtensorMap* out, const void* base, int nseq, int S, long long cols, int box_rows) {
-  static thread_local bool ctx_bound = false;   // driver entry point: needs a current context on THIS thread
-  if (!ctx_bound) {
-    DPRB_CHECK_CUDA(cudaFree(nullptr));
-    ctx_bound = true;
-  }
-  EncodeTiledFn fn = encode_fn();
-  DPRB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && cols % 8 == 0, "attention operand misaligned");
-  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)S, (cuuint64_t)nseq};
-  cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)S * cols * 2};
-  cuuint32_t box[3] = {64u, (cuuint32_t)box_rows, 1u};
-  cuuint32_t estr[3] = {1u, 1u, 1u};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  DPRB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(3d) failed with CUresult %d", (int)r);
-  return 0;
+  const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)S, (cuuint64_t)nseq};
+  const cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)S * cols * 2};
+  const cuuint32_t box[3] = {64u, (cuuint32_t)box_rows, 1u};
+  return encode_tmap(out, "attention", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, base, dims, strides, box,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 
 namespace {

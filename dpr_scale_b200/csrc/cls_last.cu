@@ -45,11 +45,6 @@ __device__ __forceinline__ void store_row64_scaled(bf16* p, const float (&v)[64]
     *reinterpret_cast<uint4*>(p + i * 8) = q;
   }
 }
-__device__ __forceinline__ float drop_mul1(const Drop& d, uint32_t r, uint32_t c) {
-  float m0, m1;
-  d.mul2(r, c & ~1u, m0, m1);
-  return (c & 1u) ? m1 : m0;
-}
 
 // ctx_cls[seq, h*64 + d] = sum_j softmax_j(q_0 . k_j / 8 + mask_j) v_j[d];  probs[(seq*heads+h)*S + j] saved (fp32).
 // MAXK: keys per lane (S <= 32 * MAXK).  MAXK = 16 asks for one CTA per SM so that its 16-key rows fit in registers
@@ -89,7 +84,7 @@ attn_cls_fwd_kernel(const bf16* __restrict__ qkv, const int32_t* __restrict__ at
     s[i] *= inv;
     if (j < S && probs != nullptr) probs[(long long)prob * S + j] = s[i];
     pd[i] = s[i];
-    if (drop.on() && j < S) pd[i] *= drop_mul1(drop, (uint32_t)(prob * S), (uint32_t)j);  // query row 0 of this problem
+    if (drop.on() && j < S) pd[i] *= drop_one(drop, (uint32_t)(prob * S), (uint32_t)j);  // query row 0 of this problem
   }
   // o[d] for d = 2*lane, 2*lane+1: coalesced 128-byte reads of V rows, p_j broadcast from its owner lane
   float o0 = 0.f, o1 = 0.f;
@@ -132,7 +127,7 @@ attn_cls_bwd_kernel(const bf16* __restrict__ qkv, const float* __restrict__ prob
     p[i] = 0.f; pd[i] = 0.f; dpm[i] = 0.f;
     if (j < S) {
       p[i] = probs[(long long)prob * S + j];
-      const float mj = drop.on() ? drop_mul1(drop, (uint32_t)(prob * S), (uint32_t)j) : 1.f;
+      const float mj = drop.on() ? drop_one(drop, (uint32_t)(prob * S), (uint32_t)j) : 1.f;
       pd[i] = p[i] * mj;
       dpm[i] = dot_row64(base + (long long)j * (3 * H) + 2 * H, dO) * mj;  // dP_j = dO . v_j (masked + rescaled)
       D = fmaf(p[i], dpm[i], D);

@@ -36,7 +36,12 @@ void set_last_error(const char* fmt, ...);
     }                                                                                \
   } while (0)
 
-int num_sms();  // cached SM count of the current device
+int num_sms();  // cached SM count of the current device; -1 (with the message set) when the query fails
+// Declares `const int var` = num_sms(); a failed query makes the calling entry point return 2.  Two statements: use it
+// only as a statement of its own at block scope (never as the body of an unbraced if / for).
+#define DPRB_NUM_SMS(var)           \
+  const int var = dprb::num_sms();  \
+  if (var <= 0) return 2
 
 // Every kernel launch of the library goes through this (one call per <<<>>> / cudaLaunchKernelEx): the running total is
 // exported as dprb_launch_count() so callers can report a MEASURED launch count instead of an estimate.
@@ -51,6 +56,11 @@ void count_launch();
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
+// SWIZZLE_128B tiles (TMA and wgmma) must start 1024-byte aligned
+__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
+}
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -104,6 +114,11 @@ __device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ float lg2_approx(float x) {
+  float y;
+  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 __device__ __forceinline__ float rcp_approx(float x) {
@@ -190,6 +205,12 @@ struct Drop {
     for (int w = 0; w < 4; ++w) lanes(pair_word(x, (uint32_t)w), m[w].x, m[w].y);
   }
 };
+// keep multiplier of element (r, c) for a single column c (the pair hash covers columns c & ~1 and c | 1)
+__device__ __forceinline__ float drop_one(const Drop& d, uint32_t r, uint32_t c) {
+  float m0, m1;
+  d.mul2(r, c & ~1u, m0, m1);
+  return (c & 1u) ? m1 : m0;
+}
 inline Drop make_drop(float p, uint64_t seed, int layer, int site) {
   const uint64_t s64 = seed + (uint64_t)(layer * 8 + site + 1) * 0x9E3779B97F4A7C15ull;
   Drop d;

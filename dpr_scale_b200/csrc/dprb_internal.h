@@ -1,9 +1,30 @@
 // Internal C++ declarations shared by the kernel translation units of libdprb.so.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include "../../include/dprb.h"
 
 namespace dprb {
+
+// host.cu: a tiled tensor map of rank 2 or 3 (dims, box: innermost first; strides: bytes, rank - 1 of them), always
+// 128B-swizzled, non-interleaved, out-of-bounds elements read as zero.  Binds the primary context to the calling
+// thread first.  Returns 0, or an error code with the message set (`what` names the caller in it).
+int encode_tmap(CUtensorMap* out, const char* what, CUtensorMapDataType dtype, int rank, const void* base,
+                const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box,
+                CUtensorMapL2promotion l2);
+
+// Bump allocator over a caller-owned workspace: every buffer starts 256-byte aligned.  With a null base it only
+// measures (take returns null, off still grows), which is how the *_workspace_bytes functions size a workspace.
+struct Carve {
+  uint8_t* base;
+  long long off;
+  explicit Carve(void* b) : base(reinterpret_cast<uint8_t*>(b)), off(0) {}
+  void* take(long long bytes) {
+    void* p = base ? base + off : nullptr;
+    off += (bytes + 255) & ~255LL;
+    return p;
+  }
+};
 
 int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long long lda, long long ldb,
               long long ldd, int a_mn_major, int b_mn_major, int epilogue, const float* bias, const void* aux,

@@ -644,9 +644,7 @@ gelu_from_pre_kernel(const bf16* __restrict__ pre, bf16* __restrict__ out, long 
   }
 }
 
-int grid_for_rows(int T) {
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
+int grid_for_rows(int T, int sms) {
   long long want = ((long long)T + WARPS - 1) / WARPS;
   long long cap = (long long)sms * 4;
   return (int)(want < cap ? want : cap);
@@ -680,7 +678,8 @@ int embed_ln_fwd(const int64_t* ids, const int64_t* type_ids, const int64_t* pos
   if (int rc = check_h(H, "embed_ln_fwd")) return rc;
   if (T == 0) return 0;
   (void)vocab; (void)max_pos; (void)type_vocab;
-  const int grid = grid_for_rows(T);
+  DPRB_NUM_SMS(sms);
+  const int grid = grid_for_rows(T, sms);
 #define CALL(C) ln_fwd_kernel<C, true, false><<<grid, THREADS, 0, stream>>>(nullptr, ids, type_ids, pos_ids, word, pos, type, gamma, beta, (bf16*)y, (bf16*)y_res, stats, nullptr, 1, T, H, eps, drop, 0)
   DISPATCH_MAXC(H, CALL);
 #undef CALL
@@ -693,7 +692,8 @@ int ln_fwd(const void* z, const float* gamma, const float* beta, void* y, float*
   if (int rc = check_h(H, "ln_fwd")) return rc;
   if (T == 0) return 0;
   DPRB_REQUIRE(cls_out == nullptr || cls_stride > 0, "ln_fwd: cls_stride must be positive");
-  const int grid = grid_for_rows(T);
+  DPRB_NUM_SMS(sms);
+  const int grid = grid_for_rows(T, sms);
   if (H % 256 == 0 && !ln_generic_forced()) {   // full-width rows (the encoder's H = 768 / 1024): paired-column kernel
 #define CALLF(C)                                                                                                         \
   do {                                                                                                                   \
@@ -725,7 +725,8 @@ int ln_bwd(const void* dy, const float* dy_cls, int cls_stride, const void* z, c
   if (T == 0) return 0;
   DPRB_REQUIRE((dy != nullptr) != (dy_cls != nullptr), "ln_bwd: exactly one of dy / dy_cls must be given");
   DPRB_REQUIRE(dy_cls == nullptr || cls_stride > 0, "ln_bwd: cls_stride must be positive");
-  const int grid = grid_for_rows(T);
+  DPRB_NUM_SMS(sms);
+  const int grid = grid_for_rows(T, sms);
   const int maxc = (H + 255) / 256;
   if (dy != nullptr && H % 256 == 0 && !ln_generic_forced()) {   // dense upstream gradient, full-width rows: paired-column kernel
     size_t front = (size_t)WARPS * H * sizeof(float);
@@ -781,7 +782,8 @@ int embed_ln_bwd(const void* dy, const int64_t* ids, const int64_t* type_ids, co
   const Drop drop = make_drop(dropout_p, seed, 0, DROP_SITE_EMBED);
   if (int rc = check_h(H, "embed_ln_bwd")) return rc;
   if (T == 0) return 0;
-  const int grid = grid_for_rows(T);
+  DPRB_NUM_SMS(sms);
+  const int grid = grid_for_rows(T, sms);
   const size_t smem = (size_t)WARPS * H * sizeof(float);
 #define CALL(C) ln_bwd_kernel<C, true, false><<<grid, THREADS, smem, stream>>>((const bf16*)dy, nullptr, 1, nullptr, ids, type_ids, pos_ids, word, pos, type, stats, gamma, nullptr, dword, dpos, dtype, dgamma, dbeta, nullptr, T, H, nullptr, drop, 0)
   DISPATCH_MAXC(H, CALL);
@@ -814,8 +816,7 @@ int dropout_mask(uint8_t* out, long long rows, int cols, float p, unsigned long 
 int colsum_bf16(const void* x, long long ld, float* out, int T, int N, cudaStream_t stream) {
   DPRB_REQUIRE(N % 8 == 0 && ld % 8 == 0, "colsum: N=%d and ld=%lld must be multiples of 8", N, ld);
   if (T == 0 || N == 0) return 0;
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
+  DPRB_NUM_SMS(sms);
   const int col_blocks = (N + 255) / 256;
   int row_chunks = (sms * 4 + col_blocks - 1) / col_blocks;
   int rows_per_cta = (T + row_chunks - 1) / row_chunks;
@@ -831,8 +832,7 @@ int gelu_from_pre(const void* pre, void* out, long long n, cudaStream_t stream) 
   DPRB_REQUIRE(n % 8 == 0 && ((reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
                "gelu_from_pre: n %% 8 == 0 and 16-byte aligned buffers required");
   if (n == 0) return 0;
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
+  DPRB_NUM_SMS(sms);
   const long long n8 = n / 8;
   const long long want = (n8 + 255) / 256;
   gelu_from_pre_kernel<<<(int)(want < (long long)sms * 8 ? want : (long long)sms * 8), 256, 0, stream>>>((const bf16*)pre, (bf16*)out, n8);

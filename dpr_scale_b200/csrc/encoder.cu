@@ -12,17 +12,6 @@
 namespace dprb {
 namespace {
 
-struct Carve {
-  uint8_t* base;
-  long long off;
-  explicit Carve(void* b) : base(reinterpret_cast<uint8_t*>(b)), off(0) {}
-  void* take(long long bytes) {
-    void* p = base ? base + off : nullptr;
-    off += (bytes + 255) & ~255LL;
-    return p;
-  }
-};
-
 struct LayerActs {
   bf16 *qkv, *ctx, *z1, *x1, *hpre, *hact, *z2, *out;
   float *lse, *stats1, *stats2;

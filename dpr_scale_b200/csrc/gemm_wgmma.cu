@@ -246,7 +246,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                  const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B needs 1024-byte aligned tiles
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   uint8_t* staging = smem + STAGES * STAGE_BYTES;                                     // [NUM_CONSUMERS][STG_BYTES]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + NUM_CONSUMERS * STG_BYTES);   // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                                // [STAGES]
@@ -393,44 +393,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 }
 
 // ---------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
-// Row-major bf16 matrix [rows, cols] with leading dimension ld (elements); box = [box_rows, 64 cols], 128B swizzle.
+// Row-major 16-bit matrix [rows, cols] with leading dimension ld (elements); box = [box_rows, 64 cols], 128B swizzle.
+// Encoded as BFLOAT16 for fp16 operands too: TMA only moves the bytes.
 int make_tmap(CUtensorMap* out, const void* base, long long rows, long long cols, long long ld, int box_rows) {
-  static thread_local bool ctx_bound = false;   // driver entry point: needs a current context on THIS thread
-  if (!ctx_bound) {
-    DPRB_CHECK_CUDA(cudaFree(nullptr));
-    ctx_bound = true;
-  }
-  EncodeTiledFn fn = get_encode_fn();
-  DPRB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "gemm operand base %p not 16-byte aligned", base);
   DPRB_REQUIRE((ld * 2) % 16 == 0, "gemm operand leading dimension %lld not a multiple of 8 elements", ld);
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  DPRB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (rows=%lld cols=%lld ld=%lld)",
-               (int)r, rows, cols, ld);
-  return 0;
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  const cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+  return encode_tmap(out, "gemm", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, dims, strides, box,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 // ---- optional live profiling: CUDA events around every GEMM launch (bench.py's roofline leg) ----
@@ -499,7 +471,7 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   p.num_m_blocks = (M + BLOCK_M - 1) / BLOCK_M;
   p.num_n_blocks = (N + BLOCK_N - 1) / BLOCK_N;
   p.k_blocks_total = (K + BLOCK_K - 1) / BLOCK_K;
-  const int sms = num_sms();
+  DPRB_NUM_SMS(sms);
   const int tiles = p.num_m_blocks * p.num_n_blocks;
   if (epilogue != DPRB_EPI_F32_ATOMIC_ADD) splits = 1;
   else if (splits <= 0) splits = choose_splits(tiles, p.k_blocks_total, sms);

@@ -107,9 +107,7 @@ uncast_kernel(const bf16* __restrict__ src, float* __restrict__ dst, long long n
   }
 }
 
-int stream_grid(long long n4) {
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
+int stream_grid(long long n4, int sms) {
   long long want = (n4 + 255) / 256;
   long long cap = (long long)sms * 8;
   if (want < 1) want = 1;
@@ -121,7 +119,8 @@ int stream_grid(long long n4) {
 int sumsq_f32(const float* g, long long n, float* out, cudaStream_t stream) {
   DPRB_REQUIRE(n >= 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0, "sumsq: buffer must be 16-byte aligned");
   if (n == 0) return 0;
-  sumsq_kernel<<<stream_grid(n >> 2), 256, 0, stream>>>(g, n, out);
+  DPRB_NUM_SMS(sms);
+  sumsq_kernel<<<stream_grid(n >> 2, sms), 256, 0, stream>>>(g, n, out);
   DPRB_LAUNCH_CHECK();
   return 0;
 }
@@ -134,12 +133,13 @@ int adamw_step(float* p, const float* g, float* m, float* v, void* shadow, long 
                  reinterpret_cast<uintptr_t>(v)) & 15) == 0 && (reinterpret_cast<uintptr_t>(shadow) & 7) == 0,
                "adamw_step: arenas must be 16-byte aligned");
   if (n == 0) return 0;
+  DPRB_NUM_SMS(sms);
   AdamArgs a;
   a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.wd = wd;
   a.bc1 = 1.f - powf(beta1, (float)step);
   a.bc2_rsqrt = 1.f / sqrtf(1.f - powf(beta2, (float)step));
   a.grad_scale = grad_scale; a.max_norm = max_norm;
-  adamw_kernel<<<stream_grid(n >> 2), 256, 0, stream>>>(p, g, m, v, (bf16*)shadow, n, a, sumsq);
+  adamw_kernel<<<stream_grid(n >> 2, sms), 256, 0, stream>>>(p, g, m, v, (bf16*)shadow, n, a, sumsq);
   DPRB_LAUNCH_CHECK();
   return 0;
 }
@@ -148,7 +148,8 @@ int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t stream)
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0,
                "cast_f32_bf16: buffers must be 16/8-byte aligned");
   if (n == 0) return 0;
-  cast_kernel<<<stream_grid(n >> 2), 256, 0, stream>>>(src, (bf16*)dst, n);
+  DPRB_NUM_SMS(sms);
+  cast_kernel<<<stream_grid(n >> 2, sms), 256, 0, stream>>>(src, (bf16*)dst, n);
   DPRB_LAUNCH_CHECK();
   return 0;
 }
@@ -157,7 +158,8 @@ int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t stream)
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(dst) & 15) == 0 && (reinterpret_cast<uintptr_t>(src) & 7) == 0,
                "cast_bf16_f32: buffers must be 8/16-byte aligned");
   if (n == 0) return 0;
-  uncast_kernel<<<stream_grid(n >> 2), 256, 0, stream>>>((const bf16*)src, dst, n);
+  DPRB_NUM_SMS(sms);
+  uncast_kernel<<<stream_grid(n >> 2, sms), 256, 0, stream>>>((const bf16*)src, dst, n);
   DPRB_LAUNCH_CHECK();
   return 0;
 }

@@ -206,17 +206,6 @@ score_ce_bwd_kernel(const float* __restrict__ logits, const float* __restrict__ 
   }
 }
 
-int sm_count() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
-  }
-  return sms;
-}
-
 }  // namespace
 
 int score_ce_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
@@ -225,6 +214,7 @@ int score_ce_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
   DPRB_REQUIRE(Q >= 0 && C > 0 && d > 0, "score_ce_fwd: bad shape Q=%d C=%d d=%d", Q, C, d);
   DPRB_REQUIRE(lse != nullptr, "score_ce_fwd: lse output required");
   if (Q == 0) return 0;
+  DPRB_NUM_SMS(sms);
   const size_t smem = (size_t)(QB * d + FWD_WARPS * QB * 3) * sizeof(float);
   DPRB_REQUIRE(smem <= 200 * 1024, "score_ce_fwd: embedding dim %d too large", d);
   static bool attr = false;
@@ -238,7 +228,7 @@ int score_ce_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
   const int step = FWD_WARPS * CW;
   int splits = 1;
   if (logits != nullptr) {
-    splits = (4 * sm_count() + row_blocks - 1) / row_blocks;
+    splits = (4 * sms + row_blocks - 1) / row_blocks;
     const int max_splits = (C + step - 1) / step;
     splits = splits < 1 ? 1 : (splits > max_splits ? max_splits : splits);
   }
@@ -262,11 +252,12 @@ int score_ce_bwd(const float* q, const float* c, const float* logits, const int6
   DPRB_REQUIRE(q0 >= 0 && nq >= 0 && q0 + nq <= Q && c0 >= 0 && nc >= 0 && c0 + nc <= C,
                "score_ce_bwd: local ranges out of bounds (q0=%d nq=%d c0=%d nc=%d)", q0, nq, c0, nc);
   DPRB_REQUIRE(logits != nullptr && lse != nullptr, "score_ce_bwd: logits and lse from forward required");
+  DPRB_NUM_SMS(sms);
   const float scale = grad_scale * inv_t / (float)Q;  // d(mean CE)/d(logit) * d(logit)/d(q.c)
   // split the reduction dimension until there are ~2 CTAs per SM (dq at 8 GPUs: 16 x 3 CTAs reducing 8192 columns)
   auto launch = [&](auto kern, const float* X, float* out, int a0, int na, int nb) -> int {
     const int base = ((na + AB - 1) / AB) * ((d + 255) / 256);
-    int z = (2 * sm_count() + base - 1) / base;
+    int z = (2 * sms + base - 1) / base;
     const int max_z = (nb + 4 * BT - 1) / (4 * BT);
     z = z < 1 ? 1 : (z > max_z ? max_z : z);
     const int per = ((nb + z - 1) / z + BT - 1) / BT * BT;

@@ -17,8 +17,6 @@
 // Backward recomputes tiles instead of reading stored logits: one launch rebuilds W = softmax - onehot for the local
 // row block [nq x C] and the local column block [Q x nc] (bf16 hi + lo), and dq = W_rows c, dc = W_cols^T q run as
 // split-K launches of the encoder's GEMM (fp32 atomic accumulate) on the h / m parts.
-#include <cstdio>
-#include <cstdlib>
 #include "common.cuh"
 #include "dprb_internal.h"
 
@@ -61,20 +59,7 @@ struct ScoreParams {
   const float* lse_in;
   Region reg[2];
   int n_regions;
-  unsigned long long* dbg;   // DPRB_SCORE_DBG=1: per-CTA role timestamps [gridDim.x][8] (diagnostics only)
 };
-__device__ __forceinline__ unsigned long long gtime() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-__device__ __forceinline__ float lg2_approx(float x) {
-  float y;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 
 // two-way bf16 split of fp32 data: out[0] = h = bf16(x), out[1] = m = bf16(x - h)  (part stride n elements)
 __global__ void __launch_bounds__(256)
@@ -101,7 +86,7 @@ template <int MODE>   // 0: forward (row statistics, optional logits)   1: W til
 __global__ void __launch_bounds__(THREADS, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_c, const ScoreParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   float* sAcc = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);    // [128][ACC_LD]
   float* sMask = sAcc + TM * ACC_LD;                                        // [2][128]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sMask + 256);
@@ -130,7 +115,6 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   if (warp == 0) {
     if (lane == 0) {
-      if (p.dbg) p.dbg[blockIdx.x * 8 + 0] = gtime();
       int stage = 0;
       uint32_t phase = 0;
       for (int t = t_begin; t < t_end; ++t) {
@@ -149,7 +133,6 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
-      if (p.dbg) p.dbg[blockIdx.x * 8 + 1] = gtime();
     }
     __syncwarp();
   } else if (warp >= 4) {
@@ -258,16 +241,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           if (lane == 0) mbar_arrive(&empty_bar[stage]);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        // accumulator -> shared memory, so that each thread can read the row it owns
-        const int r0 = quarter * 16 + (lane >> 2), q4 = lane & 3;
-#pragma unroll
-        for (int c = 0; c < TN / 8; ++c) {
-          float* a0 = sAcc + r0 * ACC_LD + 8 * c + 2 * q4;
-          *reinterpret_cast<float2*>(a0) = make_float2(d0[4 * c], d0[4 * c + 1]);
-          *reinterpret_cast<float2*>(a0 + 8 * ACC_LD) = make_float2(d0[4 * c + 2], d0[4 * c + 3]);
-          *reinterpret_cast<float2*>(a0 + 64 * ACC_LD) = make_float2(d1[4 * c], d1[4 * c + 1]);
-          *reinterpret_cast<float2*>(a0 + 72 * ACC_LD) = make_float2(d1[4 * c + 2], d1[4 * c + 3]);
-        }
+        store_acc_128x128<ACC_LD>(sAcc, d0, d1, quarter, lane);   // each thread then reads the row it owns
       }
       named_bar_sync(3, EPI_THREADS);
       const float* arow = sAcc + tid * ACC_LD;
@@ -363,52 +337,19 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       acc ^= 1;
     }
     if (MODE == 0 && cur_rb >= 0) flush(cur_rb);
-    if (p.dbg && tid == 0) p.dbg[blockIdx.x * 8 + 3] = gtime();
   }
 
   __syncthreads();
-  if (warp == 2 && p.dbg && lane == 0) p.dbg[blockIdx.x * 8 + 4] = gtime();
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
 }
 
 // bf16 [2 parts][rows][d]; box = [1][128 rows][64 cols], 128B swizzle; rows / columns beyond the extent are zero-filled
 int make_tmap_parts(CUtensorMap* out, const void* base, long long rows, long long d) {
-  // cuTensorMapEncodeTiled is a DRIVER call: it needs a current context on the calling thread.  Backward runs on
-  // autograd's worker thread, where this may be the first CUDA call of any kind - bind the primary context first.
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) {
-    DPRB_CHECK_CUDA(cudaFree(nullptr));
-    ctx_bound = true;
-  }
-  EncodeTiledFn fn = encode_fn();
-  DPRB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
-  cuuint64_t dims[3] = {(cuuint64_t)d, (cuuint64_t)rows, 2};
-  cuuint64_t strides[2] = {(cuuint64_t)d * 2, (cuuint64_t)rows * d * 2};
-  cuuint32_t box[3] = {64u, 128u, 1u};
-  cuuint32_t estr[3] = {1u, 1u, 1u};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  DPRB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(score) failed with CUresult %d", (int)r);
-  return 0;
+  const cuuint64_t dims[3] = {(cuuint64_t)d, (cuuint64_t)rows, 2};
+  const cuuint64_t strides[2] = {(cuuint64_t)d * 2, (cuuint64_t)rows * d * 2};
+  const cuuint32_t box[3] = {64u, 128u, 1u};
+  return encode_tmap(out, "score", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, base, dims, strides, box,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
-
-inline long long al256(long long x) { return (x + 255) & ~255LL; }
 
 struct ScoreWs {
   bf16 *q3, *c3;
@@ -422,20 +363,18 @@ struct ScoreWs {
 
 ScoreWs plan(void* base, int Q, int C, int d, int nq, int nc) {
   ScoreWs w;
-  uint8_t* b = reinterpret_cast<uint8_t*>(base);
-  long long off = 0;
-  auto take = [&](long long bytes) { uint8_t* ptr = b ? b + off : nullptr; off += al256(bytes); return ptr; };
+  Carve cv(base);
   w.n_rb = (Q + TM - 1) / TM; w.n_cb = (C + TN - 1) / TN; w.Qpad = w.n_rb * TM;
-  w.q3 = (bf16*)take(2LL * Q * d * 2);
-  w.c3 = (bf16*)take(2LL * C * d * 2);
-  w.part = (float*)take(3LL * w.n_cb * w.Qpad * 4);
-  w.counters = (int*)take((long long)w.n_rb * 4);
+  w.q3 = (bf16*)cv.take(2LL * Q * d * 2);
+  w.c3 = (bf16*)cv.take(2LL * C * d * 2);
+  w.part = (float*)cv.take(3LL * w.n_cb * w.Qpad * 4);
+  w.counters = (int*)cv.take((long long)w.n_rb * 4);
   w.ld_wr = (C + 7) & ~7LL; w.ld_wc = ((long long)nc + 7) & ~7LL;
-  w.wr_hi = (bf16*)take((long long)nq * w.ld_wr * 2);
-  w.wr_lo = (bf16*)take((long long)nq * w.ld_wr * 2);
-  w.wc_hi = (bf16*)take((long long)Q * w.ld_wc * 2);
-  w.wc_lo = (bf16*)take((long long)Q * w.ld_wc * 2);
-  w.bytes = off;
+  w.wr_hi = (bf16*)cv.take((long long)nq * w.ld_wr * 2);
+  w.wr_lo = (bf16*)cv.take((long long)nq * w.ld_wr * 2);
+  w.wc_hi = (bf16*)cv.take((long long)Q * w.ld_wc * 2);
+  w.wc_lo = (bf16*)cv.take((long long)Q * w.ld_wc * 2);
+  w.bytes = cv.off;
   return w;
 }
 
@@ -449,9 +388,7 @@ int set_attr() {
   return 0;
 }
 
-int grid_for(long long n4) {
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
+int grid_for(long long n4, int sms) {
   long long want = (n4 + 255) / 256;
   if (want < 1) want = 1;
   return (int)(want < (long long)sms * 4 ? want : (long long)sms * 4);
@@ -475,10 +412,11 @@ int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
   DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= w.bytes && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
                "score_tc_fwd: workspace missing, misaligned or too small (%lld < %lld)", workspace_bytes, w.bytes);
   if (int rc = set_attr()) return rc;
+  DPRB_NUM_SMS(sms);
   const long long nqd = (long long)Q * d, ncd = (long long)C * d;
-  split2_kernel<<<grid_for(nqd >> 2), 256, 0, stream>>>(q, w.q3, nqd);
+  split2_kernel<<<grid_for(nqd >> 2, sms), 256, 0, stream>>>(q, w.q3, nqd);
   DPRB_LAUNCH_CHECK();
-  split2_kernel<<<grid_for(ncd >> 2), 256, 0, stream>>>(c, w.c3, ncd);
+  split2_kernel<<<grid_for(ncd >> 2, sms), 256, 0, stream>>>(c, w.c3, ncd);
   DPRB_LAUNCH_CHECK();
   DPRB_CHECK_CUDA(cudaMemsetAsync(w.counters, 0, (size_t)w.n_rb * 4, stream));
   CUtensorMap tq, tc;
@@ -490,30 +428,9 @@ int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
   p.lse = lse; p.loss_sum = loss_sum; p.logits = logits; p.part = w.part; p.counters = w.counters; p.Qpad = w.Qpad;
   p.n_regions = 1;
   p.reg[0] = Region{0, Q, 0, C, w.n_rb, w.n_cb, nullptr, nullptr, 0};
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
   const int tiles = w.n_rb * w.n_cb;
-  static unsigned long long* dbg = nullptr;
-  static const bool want_dbg = getenv("DPRB_SCORE_DBG") != nullptr;
-  if (want_dbg && dbg == nullptr) DPRB_CHECK_CUDA(cudaMalloc(&dbg, 148 * 8 * 8));
-  p.dbg = want_dbg ? dbg : nullptr;
-  const int grid = tiles < sms ? tiles : sms;
-  score_tc_kernel<0><<<grid, THREADS, SMEM_BYTES, stream>>>(tq, tc, p);
+  score_tc_kernel<0><<<tiles < sms ? tiles : sms, THREADS, SMEM_BYTES, stream>>>(tq, tc, p);
   DPRB_LAUNCH_CHECK();
-  if (want_dbg) {
-    static int calls = 0;
-    if (++calls == 3) {   // a warmed-up launch
-      unsigned long long h[148 * 8];
-      DPRB_CHECK_CUDA(cudaStreamSynchronize(stream));
-      DPRB_CHECK_CUDA(cudaMemcpy(h, dbg, sizeof(h), cudaMemcpyDeviceToHost));
-      unsigned long long t0 = ~0ull;
-      for (int i = 0; i < grid; ++i) if (h[i * 8] < t0) t0 = h[i * 8];
-      for (int i = 0; i < grid; ++i)
-        fprintf(stderr, "[score dbg] cta %3d start %7.1f producer_end %7.1f mma_end %7.1f epi_end %7.1f dealloc %7.1f us\n", i,
-                (h[i * 8] - t0) / 1e3, (h[i * 8 + 1] - t0) / 1e3, (h[i * 8 + 2] - t0) / 1e3, (h[i * 8 + 3] - t0) / 1e3,
-                (h[i * 8 + 4] - t0) / 1e3);
-    }
-  }
   return 0;
 }
 
@@ -541,8 +458,7 @@ int score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const int64_
   p.n_regions = nreg;
   int tiles = 0;
   for (int i = 0; i < nreg; ++i) tiles += p.reg[i].n_rb * p.reg[i].n_cb;
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
+  DPRB_NUM_SMS(sms);
   score_tc_kernel<1><<<tiles < sms ? tiles : sms, THREADS, SMEM_BYTES, stream>>>(tq, tc, p);
   DPRB_LAUNCH_CHECK();
   const float scale = grad_scale * inv_t / (float)Q;        // d(mean CE)/d(logit) * d(logit)/d(q.c)

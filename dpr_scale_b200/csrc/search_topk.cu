@@ -19,7 +19,6 @@
 // Ranking is by fp32-accumulated score, ties broken towards the lower index (torch.topk leaves tie order
 // unspecified).  Results are exact for the fp32 scores: no approximation, no score quantisation.
 #include <cstdint>
-#include <cstdlib>
 #include "common.cuh"
 #include "dprb_internal.h"
 
@@ -58,17 +57,11 @@ struct SearchParams {
   int* counts;          // [gridDim.x][gridDim.y * 128]
   uint32_t* bounds;     // [gridDim.x][gridDim.y * 128] ordered-uint of each partition's m-th best score (0 = none yet)
   int m_track;          // m = ceil(k / partitions) if <= 8, else 0 (cross-partition bound disabled)
-  int pf_ahead;         // corpus k-block boxes prefetched into L2 ahead of the shared-memory ring (0 = off)
   int f16;              // operands are fp16 (else bf16)
   int rank_f16;         // rank by the fp16-ROUNDED score: the reference's einsum on fp16 tensors returns fp16
                         // (run_retrieval_pytorch.py:150-151), so its topk orders fp16 values; ties go to the lower row id
 };
 
-// TMA prefetch of one box into L2 (no shared-memory destination, no barrier)
-__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ uint32_t ord_u32(float v) {   // monotone float -> unsigned
   const uint32_t u = __float_as_uint(v);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
@@ -160,7 +153,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
                    const SearchParams p) {
   constexpr uint32_t CAP = 32 * EPL;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_BYTES;
   float* sAcc = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [QT][ACC_LD]
@@ -190,25 +183,11 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   if (warp == 0) {
     // ---------------- TMA producer: query tile (L2-resident) + corpus tile (HBM stream) per k-block
     if (lane == 0) {
-      // Optional: pull corpus boxes into L2 pf_ahead k-blocks ahead of the 4-stage ring (DPRB_SEARCH_PF; off by
-      // default).
       int stage = 0;
       uint32_t phase = 0;
-      const long long items = (t1 - t0) * p.kblocks;
-      long long pf = 0;                                    // next (tile, k-block) item to prefetch
-      int pf_kb = 0;
-      long long pf_t = t0;
-      auto prefetch_until = [&](long long upto) {
-        for (; pf < upto && pf < items; ++pf) {
-          tma_prefetch_l2_2d(&tm_c, pf_kb * BK, (int)(pf_t * CT));
-          if (++pf_kb == p.kblocks) { pf_kb = 0; ++pf_t; }
-        }
-      };
-      long long n = 0;
       for (long long t = t0; t < t1; ++t) {
         const int row0 = (int)(t * CT);
-        for (int kb = 0; kb < p.kblocks; ++kb, ++n) {
-          if (p.pf_ahead > 0) prefetch_until(n + p.pf_ahead);
+        for (int kb = 0; kb < p.kblocks; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
           tma_load_2d(smem_a + stage * A_BYTES, &tm_q, &full_bar[stage], kb * BK, q0);
@@ -269,15 +248,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
         // the previous tile's rows have all been read (barrier at the end of the loop body)
-        const int r0 = quarter * 16 + (lane >> 2), q4 = lane & 3;
-#pragma unroll
-        for (int c = 0; c < CT / 8; ++c) {
-          float* a0 = sAcc + r0 * ACC_LD + 8 * c + 2 * q4;
-          *reinterpret_cast<float2*>(a0) = make_float2(d0[4 * c], d0[4 * c + 1]);
-          *reinterpret_cast<float2*>(a0 + 8 * ACC_LD) = make_float2(d0[4 * c + 2], d0[4 * c + 3]);
-          *reinterpret_cast<float2*>(a0 + 64 * ACC_LD) = make_float2(d1[4 * c], d1[4 * c + 1]);
-          *reinterpret_cast<float2*>(a0 + 72 * ACC_LD) = make_float2(d1[4 * c + 2], d1[4 * c + 3]);
-        }
+        store_acc_128x128<ACC_LD>(sAcc, d0, d1, quarter, lane);
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
       const long long rem = p.N - t * CT;
@@ -455,68 +426,36 @@ __global__ void pack_keys_kernel(const float* __restrict__ scores, u64* keys, lo
   if (i < n) keys[i] = make_key(scores[i], (uint32_t)(i % total));
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
 // row-major 16-bit matrix [rows, d]; box = [box_rows, 64 cols]; rows / cols past the end read as zero
 int make_tmap(CUtensorMap* out, const void* base, long long rows, int d, int box_rows, int dtype) {
-  EncodeTiledFn fn = encode_fn();
-  DPRB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t dims[2] = {(cuuint64_t)d, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)d * 2};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = fn(out, dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                  const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  DPRB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (rows=%lld d=%d)", (int)r, rows, d);
-  return 0;
-}
-
-int num_sms_cached() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return sms;
+  const cuuint64_t dims[2] = {(cuuint64_t)d, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)d * 2};
+  const cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+  return encode_tmap(out, "search", dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
+                     base, dims, strides, box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 int cap_for_k(int k) { return k <= 256 ? 512 : 2048; }
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 struct WsLayout {
-  size_t queues, counts, bounds, scratch, total;
-  long long scratch_per_query;
+  u64* queues;
+  int* counts;
+  uint32_t* bounds;
+  u64* scratch;           // null when every query's candidates fit the selection kernel's shared memory
+  long long scratch_per_query, total;
 };
-WsLayout ws_layout(long long Q, int k) {
-  const int sms = num_sms_cached() > 0 ? num_sms_cached() : 148;
+WsLayout ws_layout(void* base, long long Q, int k, int sms) {
   const long long slots = (long long)sms * QT;                      // parts * qtiles * 128 <= sms * 128 per launch
+  Carve c(base);
   WsLayout w;
-  w.queues = 0;
-  size_t off = align256((size_t)slots * cap_for_k(k) * sizeof(u64));
-  w.counts = off;
-  off += align256((size_t)slots * sizeof(int));
-  w.bounds = off;
-  off += align256((size_t)slots * sizeof(uint32_t));
-  w.scratch = off;
+  w.queues = (u64*)c.take(slots * cap_for_k(k) * (long long)sizeof(u64));
+  w.counts = (int*)c.take(slots * (long long)sizeof(int));
+  w.bounds = (uint32_t*)c.take(slots * (long long)sizeof(uint32_t));
   w.scratch_per_query = (long long)sms * k;                         // parts <= sms lists of <= k keys
   const long long qb = Q < (long long)MAX_QTILES * QT ? Q : (long long)MAX_QTILES * QT;
-  if (w.scratch_per_query > SEL_SMEM_KEYS) off += align256((size_t)qb * w.scratch_per_query * sizeof(u64));
-  w.total = off;
+  w.scratch = w.scratch_per_query > SEL_SMEM_KEYS ? (u64*)c.take(qb * w.scratch_per_query * (long long)sizeof(u64))
+                                                  : nullptr;
+  w.total = c.off;
   return w;
 }
 
@@ -540,7 +479,10 @@ int kpad_for(int k) {
 
 }  // namespace
 
-long long search_workspace_bytes(long long Q, int k) { return (long long)ws_layout(Q, k).total; }
+long long search_workspace_bytes(long long Q, int k) {
+  const int sms = num_sms();
+  return sms > 0 ? ws_layout(nullptr, Q, k, sms).total : -1;
+}
 
 int search_topk(const void* queries, const void* corpus, int dtype, long long Q, long long N, int d, int k,
                 long long index_offset, float* out_scores, long long* out_index, void* workspace,
@@ -555,14 +497,10 @@ int search_topk(const void* queries, const void* corpus, int dtype, long long Q,
   DPRB_REQUIRE(d % 8 == 0, "search: d=%d must be a multiple of 8 (16-byte rows for TMA)", d);
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(queries) & 15) == 0 && (reinterpret_cast<uintptr_t>(corpus) & 15) == 0,
                "search: operands must be 16-byte aligned");
-  const WsLayout w = ws_layout(Q, k);
-  DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= (long long)w.total,
-               "search: workspace %lld B < required %zu B", workspace_bytes, w.total);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  u64* queues = reinterpret_cast<u64*>(ws + w.queues);
-  int* counts = reinterpret_cast<int*>(ws + w.counts);
-  uint32_t* bounds = reinterpret_cast<uint32_t*>(ws + w.bounds);
-  u64* scratch = w.scratch_per_query > SEL_SMEM_KEYS ? reinterpret_cast<u64*>(ws + w.scratch) : nullptr;
+  DPRB_NUM_SMS(sms);
+  const WsLayout w = ws_layout(workspace, Q, k, sms);
+  DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= w.total,
+               "search: workspace %lld B < required %lld B", workspace_bytes, w.total);
 
   static bool attr_set = false;
   if (!attr_set) {
@@ -570,7 +508,6 @@ int search_topk(const void* queries, const void* corpus, int dtype, long long Q,
     DPRB_CHECK_CUDA(cudaFuncSetAttribute(search_topk_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     attr_set = true;
   }
-  const int sms = num_sms_cached();
   const int cap = cap_for_k(k);
   const long long tiles = (N + CT - 1) / CT;
   CUtensorMap tc;
@@ -590,36 +527,36 @@ int search_topk(const void* queries, const void* corpus, int dtype, long long Q,
     if (int rc = make_tmap(&tq, qptr, Qb, d, QT, dtype)) return rc;
     SearchParams sp;
     sp.N = N; sp.Q = Qb; sp.d = d; sp.k = k; sp.kblocks = (d + BK - 1) / BK;
-    sp.tiles = tiles; sp.tiles_per_part = tpp; sp.queues = queues; sp.counts = counts;
+    sp.tiles = tiles; sp.tiles_per_part = tpp; sp.queues = w.queues; sp.counts = w.counts;
     sp.f16 = dtype == 0 ? 1 : 0;
     sp.rank_f16 = rank_f16;
     const long long m = (k + parts - 1) / parts;
-    sp.bounds = bounds;
-    {
-      const char* e = getenv("DPRB_SEARCH_PF");
-      sp.pf_ahead = e != nullptr ? atoi(e) : 0;
-    }
+    sp.bounds = w.bounds;
     sp.m_track = m <= 8 ? (int)m : 0;
     if (sp.m_track > 0)
-      DPRB_CHECK_CUDA(cudaMemsetAsync(bounds, 0, (size_t)parts * nb * QT * sizeof(uint32_t), stream));
+      DPRB_CHECK_CUDA(cudaMemsetAsync(w.bounds, 0, (size_t)parts * nb * QT * sizeof(uint32_t), stream));
     dim3 grid((unsigned)parts, (unsigned)nb);
     if (cap == 512) search_topk_kernel<16><<<grid, THREADS, SMEM_BYTES, stream>>>(tq, tc, sp);
     else search_topk_kernel<64><<<grid, THREADS, SMEM_BYTES, stream>>>(tq, tc, sp);
     DPRB_LAUNCH_CHECK();
     SelectParams sl;
     const long long qpad = (long long)nb * QT;
-    sl.lists = queues; sl.counts = counts; sl.num_lists = (int)parts;
+    sl.lists = w.queues; sl.counts = w.counts; sl.num_lists = (int)parts;
     sl.list_stride = qpad * cap; sl.query_stride = cap; sl.count_stride = qpad; sl.fixed_count = 0;
     sl.k = k; sl.kpad = kpad_for(k); sl.index_offset = index_offset;
     sl.out_scores = out_scores + qbase * k; sl.out_index = out_index + qbase * k;
-    sl.scratch = scratch; sl.scratch_per_query = w.scratch_per_query;
+    sl.scratch = w.scratch; sl.scratch_per_query = w.scratch_per_query;
     sl.gather = nullptr; sl.gather_stride = 0;
     if (int rc = launch_select(sl, Qb, stream)) return rc;
   }
   return 0;
 }
 
-long long topk_merge_workspace_bytes(long long Q, int total) { return (long long)align256((size_t)Q * total * sizeof(u64)); }
+long long topk_merge_workspace_bytes(long long Q, int total) {
+  Carve c(nullptr);
+  c.take(Q * total * (long long)sizeof(u64));
+  return c.off;
+}
 
 int topk_merge(const float* scores, const long long* index, long long Q, int total, int k, float* out_scores,
                long long* out_index, void* workspace, long long workspace_bytes, cudaStream_t stream) {

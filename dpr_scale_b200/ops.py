@@ -18,10 +18,6 @@ def launch_count():
     return int(_lib.load().dprb_launch_count())
 
 
-def _count(n=1):  # kept as a no-op hook: launches are counted in C (dprb_launch_count), not estimated here
-    pass
-
-
 def _ptr(t):
     if t is None:
         return None
@@ -40,7 +36,6 @@ def gemm(a, b, out, M, N, K, lda, ldb, ldd, a_mn=False, b_mn=False, epilogue=EPI
                              _ptr(bias), _ptr(aux), ld_aux, _ptr(out2), float(alpha), splits, _ptr(colsum),
                              float(dropout_p), int(drop_seed), _stream()),
           "dprb_gemm_bf16")
-    _count()
     return out
 
 
@@ -63,7 +58,6 @@ def embed_ln_fwd(ids, type_ids, pos_ids, word, pos, typ, gamma, beta, eps, dropo
                                         _ptr(gamma), _ptr(beta), _ptr(y), _ptr(stats), T, H, word.shape[0],
                                         pos.shape[0], typ.shape[0], float(eps), float(dropout_p), int(seed), _ptr(y_res),
                                         _stream()), "dprb_embed_ln_fwd")
-    _count()
     return y, stats
 
 
@@ -75,7 +69,6 @@ def embed_ln_bwd(dy, ids, type_ids, pos_ids, word, pos, typ, gamma, stats, dword
                                         _ptr(typ), _ptr(gamma), _ptr(stats), _ptr(dword), _ptr(dpos), _ptr(dtyp),
                                         _ptr(dgamma), _ptr(dbeta), T, H, float(dropout_p), int(seed), _stream()),
           "dprb_embed_ln_bwd")
-    _count()
 
 
 def ln_fwd(z, gamma, beta, eps, cls_stride=0, y_res=None):
@@ -89,7 +82,6 @@ def ln_fwd(z, gamma, beta, eps, cls_stride=0, y_res=None):
     check(_lib.load().dprb_ln_fwd(_ptr(z), _ptr(gamma), _ptr(beta), _ptr(y), _ptr(stats), _ptr(cls),
                                   cls_stride if cls_stride else 1, T, H, float(eps), int(z.dtype == torch.float16),
                                   _ptr(y_res), _stream()), "dprb_ln_fwd")
-    _count()
     return y, stats, cls
 
 
@@ -100,7 +92,6 @@ def ln_bwd(dy, z, stats, gamma, dgamma, dbeta, dbias=None, dy_cls=None, cls_stri
     check(_lib.load().dprb_ln_bwd(_ptr(dy), _ptr(dy_cls), cls_stride, _ptr(z), _ptr(stats), _ptr(gamma), _ptr(dz),
                                   _ptr(dgamma), _ptr(dbeta), _ptr(dbias), T, H, _ptr(dzm), float(dropout_p),
                                   int(site_seed), int(z.dtype == torch.float16), _stream()), "dprb_ln_bwd")
-    _count()
     return (dz, dzm) if dropout_p > 0 else dz
 
 
@@ -125,7 +116,6 @@ def gelu_from_pre(pre):
 def colsum(x, out):
     T, N = x.shape
     check(_lib.load().dprb_colsum_bf16(_ptr(x), x.stride(0), _ptr(out), T, N, _stream()), "dprb_colsum_bf16")
-    _count()
     return out
 
 
@@ -136,7 +126,6 @@ def attn_fwd(qkv, attn_mask, nseq, S, heads, need_lse=True, dropout_p=0.0, site_
     lse = torch.empty(nseq, heads, S, dtype=torch.float32, device=qkv.device) if need_lse else None
     check(_lib.load().dprb_attn_fwd(_ptr(qkv), _ptr(attn_mask), _ptr(ctx), _ptr(lse), nseq, S, heads, float(dropout_p),
                                     int(site_seed), _stream()), "dprb_attn_fwd")
-    _count()
     return ctx, lse
 
 
@@ -145,11 +134,7 @@ def attn_bwd(qkv, attn_mask, ctx, lse, dctx, nseq, S, heads, dbias=None, dropout
     check(_lib.load().dprb_attn_bwd(_ptr(qkv), _ptr(attn_mask), _ptr(ctx), _ptr(lse), _ptr(dctx), _ptr(dqkv),
                                     _ptr(dbias), nseq, S, heads, float(dropout_p), int(site_seed), _stream()),
           "dprb_attn_bwd")
-    _count()
     return dqkv
-
-
-import os as _os
 
 
 class ScoreCtx:
@@ -164,7 +149,7 @@ class ScoreCtx:
 
 
 def score_tc_supported(Q, C, d):
-    return bool(_lib.load().dprb_score_tc_supported(Q, C, d)) and not _os.environ.get("DPRB_SCORE_LEGACY")
+    return bool(_lib.load().dprb_score_tc_supported(Q, C, d))
 
 
 def score_fwd(q, c, col_mask, labels, inv_temperature, want_logits=False, pair_mask=None, local=None):
@@ -239,7 +224,6 @@ def score_ce_bwd(q, c, logits, labels, lse, grad_scale, inv_temperature, q0, nq,
 
 def sumsq(g, out):
     check(_lib.load().dprb_sumsq_f32(_ptr(g), g.numel(), _ptr(out), _stream()), "dprb_sumsq_f32")
-    _count()
     return out
 
 
@@ -249,12 +233,10 @@ def adamw_step(p, g, m, v, shadow, lr, beta1, beta2, eps, weight_decay, step, gr
                                       float(beta1), float(beta2), float(eps), float(weight_decay), int(step),
                                       float(grad_scale), _ptr(sumsq_buf), float(max_norm), _stream()),
           "dprb_adamw_step")
-    _count()
 
 
 def cast_f32_bf16(src, dst):
     check(_lib.load().dprb_cast_f32_bf16(_ptr(src), _ptr(dst), src.numel(), _stream()), "dprb_cast_f32_bf16")
-    _count()
     return dst
 
 
@@ -284,14 +266,16 @@ def search_topk(queries, corpus, k, index_offset=0, reference_ranking=False):
     lib = _lib.load()
     Q, d = queries.shape
     N = corpus.shape[0]
-    ws = _search_ws(lib.dprb_search_workspace_bytes(Q, int(k)), queries.device)
+    nbytes = lib.dprb_search_workspace_bytes(Q, int(k))
+    if nbytes < 0:
+        check(1, "dprb_search_workspace_bytes")
+    ws = _search_ws(nbytes, queries.device)
     scores = torch.empty(Q, k, dtype=torch.float32, device=queries.device)
     index = torch.empty(Q, k, dtype=torch.int64, device=queries.device)
     check(lib.dprb_search_topk(_ptr(queries), _ptr(corpus),
                                (1 if queries.dtype == torch.bfloat16 else 0) | (0x100 if reference_ranking else 0), Q, N, d,
                                int(k), int(index_offset), _ptr(scores), _ptr(index), _ptr(ws), ws.numel(),
                                _stream()), "dprb_search_topk")
-    _count(2 * ((Q + 1023) // 1024))
     return scores, index
 
 
@@ -306,5 +290,4 @@ def topk_merge(scores, index, k):
     out_i = torch.empty(Q, k, dtype=torch.int64, device=scores.device)
     check(lib.dprb_topk_merge(_ptr(scores), _ptr(index), Q, total, int(k), _ptr(out_s), _ptr(out_i), _ptr(ws),
                               ws.numel(), _stream()), "dprb_topk_merge")
-    _count(2)
     return out_s, out_i
