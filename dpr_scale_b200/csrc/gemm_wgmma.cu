@@ -6,10 +6,12 @@
 // 128x256 tile: warpgroups 1 and 2 own rows [0, 64) and [64, 128) (wgmma m64n256k16, 128 fp32 accumulators per
 // thread), warpgroup 0 is the TMA producer (one thread issues, setmaxnreg hands its registers to the consumers).  The
 // 3-stage ring of 48 KB runs across unit boundaries, so the producer loads the next unit's first k-blocks while the
-// consumers run the current unit's epilogue.  16-bit outputs go through a per-warpgroup staging slab in shared memory:
-// the fragment-layout results are written there, then each warp stores whole 512-byte rows with 16-byte stores.  The
-// aux operand (residual, gelu'(pre) or pre-activation) comes in the same way.  fp32 outputs (split-K partial sums)
-// stay fragment-layout red.global.add.v2.f32 / st.global straight from the registers.
+// consumers run the current unit's epilogue.  16-bit outputs go through a per-warpgroup staging slab in shared memory
+// laid out as the TMA box (four 64-column, 128B-swizzled subtiles): the fragment-layout results are written there and
+// one thread issues TMA stores, so the warpgroup goes straight back to the next unit's MMAs while the tile drains.  The
+// aux operand (residual, gelu'(pre) or pre-activation) is TMA-loaded into the same slab by the producer during the
+// unit's mainloop, once the previous unit's stores have read it.  fp32 outputs (split-K partial sums) stay
+// fragment-layout red.global.add.v2.f32 / st.global straight from the registers.
 //
 // Replaces, on the reference path, every torch.nn.Linear call inside HF BertLayer (QKV, attention output,
 // intermediate, output) and their autograd backward (dgrad / wgrad).
@@ -36,9 +38,10 @@ constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
 constexpr int NUM_CONSUMERS = 2;                      // warpgroups
 constexpr int NUM_THREADS = (NUM_CONSUMERS + 1) * 128; // + the producer warpgroup
 constexpr int WG_ROWS = BLOCK_M / NUM_CONSUMERS;      // 64
-// Staging slab row pitch in 16-bit elements: +16 B per row puts the 8 rows a fragment store touches on distinct banks.
-constexpr int STG_LD = BLOCK_N + 8;
-constexpr int STG_BYTES = WG_ROWS * STG_LD * 2;
+// Staging slab of one consumer warpgroup: 64 rows x 256 16-bit columns as four TMA boxes of 64 columns (128 B per row).
+constexpr int SUB_COLS = 64;
+constexpr int SUB_BYTES = WG_ROWS * SUB_COLS * 2;   // 8 KB
+constexpr int STG_BYTES = WG_ROWS * BLOCK_N * 2;    // 32 KB
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + NUM_CONSUMERS * STG_BYTES + 1024 /*align slack*/ + 128 /*barriers*/;
 static_assert(SMEM_BYTES <= 227 * 1024, "ring + staging must fit one CTA per SM");
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
@@ -53,9 +56,8 @@ struct GemmParams {
   void* D;
   long long ldd;
   const float* bias;   // [N] fp32 or null
-  const bf16* aux;     // residual (EPI_BIAS_RESIDUAL) or pre-activation (EPI_DGELU), ld = ld_aux
-  long long ld_aux;
-  bf16* out2;          // EPI_BIAS_GELU: pre-activation store, ld = ldd
+  int has_aux;         // EPI_BIAS_RESIDUAL / EPI_DGELU / EPI_DGELU_PRE: the aux tile is TMA-loaded into the slab
+  int has_out2;        // EPI_BIAS_GELU: a second output (gelu'(pre) or pre) goes to the out2 map
   float alpha;         // scale applied to the accumulator before the epilogue
   float* colsum;       // optional: colsum[n] += sum_m D(m, n) of the bf16-rounded output (bias gradients)
   Drop drop;           // EPI_BIAS_RESIDUAL only: D = dropout(acc + bias) + aux  (hidden dropout before the residual)
@@ -105,46 +107,35 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[128], uint32_t sa, uint3
 
 __device__ __forceinline__ uint32_t pack_out(float a, float b, bool f16) { return f16 ? pack_f16x2(a, b) : pack_bf16x2(a, b); }
 
-// The warpgroup's 64 x 256 slab of 16-bit values as 64 * 32 chunks of 16 B; thread t moves chunks t + 128 j, so each
-// warp covers one 512-byte row per step.  Rows >= M and columns >= N are skipped (a chunk straddling N goes element by
-// element).  Global rows and columns are 16-byte aligned: the host requires ld % 8 == 0 and 16-byte aligned bases.
-__device__ __forceinline__ void slab_store(const uint8_t* stg, uint16_t* g, long long ld, int row0, int n0, int M, int N,
-                                           int t) {
-#pragma unroll 4
-  for (int j = 0; j < WG_ROWS * BLOCK_N / 8 / 128; ++j) {
-    const int idx = t + 128 * j, r = idx >> 5, col = n0 + (idx & 31) * 8;
-    if (row0 + r >= M || col >= N) continue;
-    const uint4 v = *reinterpret_cast<const uint4*>(stg + r * (STG_LD * 2) + (idx & 31) * 16);
-    uint16_t* dst = g + (long long)(row0 + r) * ld + col;
-    if (col + 8 <= N) {
-      *reinterpret_cast<uint4*>(dst) = v;
-    } else {
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int e = 0; e < 8; ++e)
-        if (col + e < N) dst[e] = (uint16_t)(w[e >> 1] >> (16 * (e & 1)));
-    }
-  }
+// Staging slab addressing.  Subtile c / 8 holds columns [64 (c / 8), +64) as 64 rows of 128 B, 128B-swizzled the way
+// TMA reads and writes it: 16-byte chunk j of row r sits at chunk j ^ (r & 7).  The 8 rows one fragment store touches
+// thus land in 8 different chunks, on 32 distinct banks.  A thread's pairs sit in rows lr and lr + 8, which share
+// r & 7, so one base address per thread (row lr, its swizzled chunk 0, byte 4q) gives every pair with an XOR and an
+// immediate offset.  32-bit shared addresses keep that to one register: with generic pointers the compiler hoists all
+// 64 pair addresses out of the tile loop and spills them.
+__device__ __forceinline__ uint32_t slab_base(const uint8_t* stg, int lr, int q) {
+  return smem_u32(stg) + lr * 128 + ((lr & 7) << 4) + 4 * q;
 }
-__device__ __forceinline__ void slab_load(uint8_t* stg, const uint16_t* g, long long ld, int row0, int n0, int M, int N,
-                                          int t) {
-#pragma unroll 4
-  for (int j = 0; j < WG_ROWS * BLOCK_N / 8 / 128; ++j) {
-    const int idx = t + 128 * j, r = idx >> 5, col = n0 + (idx & 31) * 8;
-    if (row0 + r >= M || col >= N) continue;
-    const uint16_t* src = g + (long long)(row0 + r) * ld + col;
-    uint4 v;
-    if (col + 8 <= N) {
-      v = __ldg(reinterpret_cast<const uint4*>(src));
-    } else {
-      uint32_t w[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-      for (int e = 0; e < 8; ++e)
-        if (col + e < N) w[e >> 1] |= (uint32_t)__ldg(src + e) << (16 * (e & 1));
-      v = make_uint4(w[0], w[1], w[2], w[3]);
-    }
-    *reinterpret_cast<uint4*>(stg + r * (STG_LD * 2) + (idx & 31) * 16) = v;
-  }
+// the pair (row lr + 8h, columns 8c + 2q, +1)
+__device__ __forceinline__ uint32_t slab_pair(uint32_t base, int c, int h) {
+  return (base ^ ((c & 7) << 4)) + (c >> 3) * SUB_BYTES + h * 8 * 128;
+}
+__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v)); }
+__device__ __forceinline__ uint32_t lds32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a));
+  return v;
+}
+// Subtiles of the 64-row slab at (row0, n0) that hold any in-bounds element.  TMA clips the rest of a partial box on
+// store and zero-fills it on load.
+__device__ __forceinline__ int slab_boxes(int row0, int n0, int M, int N) {
+  return row0 < M ? min(BLOCK_N / SUB_COLS, (N - n0 + SUB_COLS - 1) / SUB_COLS) : 0;
+}
+// One thread: TMA-store the slab as one bulk group.  The caller has fenced its writes to the async proxy and synced.
+__device__ __forceinline__ void slab_tma_store(const CUtensorMap* m, const uint8_t* stg, int row0, int n0, int M, int N) {
+  const int boxes = slab_boxes(row0, n0, M, N);
+  for (int s = 0; s < boxes; ++s) tma_store_2d(m, smem_u32(stg + s * SUB_BYTES), n0 + s * SUB_COLS, row0);
+  tma_store_commit();
 }
 
 // fp32 output straight from the fragment registers: split-K partial sums (red.global.add) or a plain store + bias
@@ -175,7 +166,7 @@ __device__ __forceinline__ void epilogue_f32(const GemmParams& p, const float (&
 // a short straight run of code, where one loop branching on all of them per element pair spans ~170 KB of SASS and
 // misses the instruction cache on every tile.  EPI_BIAS_GELU leaves out2's values in acc.
 template <int EP, bool DROP, bool COLSUM>
-__device__ __forceinline__ void epilogue16(const GemmParams& p, float (&acc)[128], uint8_t* stg, int row0, int n0, int lr,
+__device__ __forceinline__ void epilogue16(const GemmParams& p, float (&acc)[128], uint32_t slab, int row0, int n0, int lr,
                                            int q, int lane) {
   const bool out_f16 = p.out_f16 != 0, aux_f16 = p.aux_f16 != 0;
 #pragma unroll
@@ -190,13 +181,13 @@ __device__ __forceinline__ void epilogue16(const GemmParams& p, float (&acc)[128
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = row0 + lr + 8 * h;
-      uint32_t* sp = reinterpret_cast<uint32_t*>(stg + (lr + 8 * h) * (STG_LD * 2) + (8 * c + 2 * q) * 2);
+      const uint32_t sp = slab_pair(slab, c, h);
       float2 v = ffma2(make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]), make_float2(p.alpha, p.alpha), b);
       if constexpr (EP == DPRB_EPI_BIAS_GELU) {
         float2 g, d;
         gelu_and_grad2(v, g, d);
         if (p.save_pre) d = v;        // lean activations: keep pre, rebuild gelu / gelu' in backward
-        *sp = pack_bf16x2(g.x, g.y);
+        sts32(sp, pack_bf16x2(g.x, g.y));
         acc[4 * c + 2 * h] = d.x;
         acc[4 * c + 2 * h + 1] = d.y;
         continue;
@@ -207,18 +198,18 @@ __device__ __forceinline__ void epilogue16(const GemmParams& p, float (&acc)[128
         v.x *= m0f; v.y *= m1f;
       }
       if constexpr (EP == DPRB_EPI_BIAS_RESIDUAL) {
-        const float2 a = unpack_16x2(*sp, aux_f16);
+        const float2 a = unpack_16x2(lds32(sp), aux_f16);
         v.x += a.x; v.y += a.y;
       } else if constexpr (EP == DPRB_EPI_DGELU) {
-        const float2 a = unpack_bf16x2(*sp);   // aux holds gelu'(pre) written by the forward epilogue
+        const float2 a = unpack_bf16x2(lds32(sp));   // aux holds gelu'(pre) written by the forward epilogue
         v.x *= a.x; v.y *= a.y;
       } else if constexpr (EP == DPRB_EPI_DGELU_PRE) {
         float2 g, d;                           // aux holds the pre-activation: derivative rebuilt (same fitted function)
-        gelu_and_grad2(unpack_bf16x2(*sp), g, d);
+        gelu_and_grad2(unpack_bf16x2(lds32(sp)), g, d);
         v.x *= d.x; v.y *= d.y;
       }
       const uint32_t o = pack_out(v.x, v.y, out_f16);
-      *sp = o;
+      sts32(sp, o);
       if (COLSUM && row < p.M && col < p.N) {   // bias gradient: sums of the bf16-rounded output
         const float2 f = unpack_bf16x2(o);
         cs0 += f.x;
@@ -243,23 +234,34 @@ __device__ __forceinline__ void epilogue16(const GemmParams& p, float (&acc)[128
 template <int A_MN, int B_MN, int F16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const GemmParams p) {
+                 const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_aux,
+                 const __grid_constant__ CUtensorMap tmap_out2, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B needs 1024-byte aligned tiles
   uint8_t* smem = align1024(smem_raw);
   uint8_t* staging = smem + STAGES * STAGE_BYTES;                                     // [NUM_CONSUMERS][STG_BYTES]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + NUM_CONSUMERS * STG_BYTES);   // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                                // [STAGES]
+  uint64_t* aux_full = empty_bar + STAGES;                                                // [NUM_CONSUMERS]
+  uint64_t* slab_empty = aux_full + NUM_CONSUMERS;                                        // [NUM_CONSUMERS]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const bool out16 = p.epilogue != DPRB_EPI_F32_ATOMIC_ADD && p.epilogue != DPRB_EPI_F32_STORE;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if (out16) tma_prefetch_desc(&tmap_d);
+    if (p.has_aux) tma_prefetch_desc(&tmap_aux);
+    if (p.has_out2) tma_prefetch_desc(&tmap_out2);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);                   // producer arrive (+ transaction bytes)
       mbar_init(&empty_bar[i], NUM_CONSUMERS * 4);  // one arrive per consumer warp
+    }
+    for (int i = 0; i < NUM_CONSUMERS; ++i) {
+      mbar_init(&aux_full[i], 1);                   // producer arrive (+ transaction bytes)
+      mbar_init(&slab_empty[i], 1);                 // the warpgroup's storing thread, once its stores have read the slab
     }
     fence_barrier_init();
   }
@@ -270,9 +272,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
     if (warp == 0 && lane == 0) {
       int stage = 0;
-      uint32_t phase = 0;
-      for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+      uint32_t phase = 0, uphase = 0;
+      for (int u = blockIdx.x; u < p.units; u += gridDim.x, uphase ^= 1) {
         const Unit w = unit_at(p, u);
+        // The aux tile goes in after this unit's first k-blocks are queued: the consumers free the slab at their second
+        // k-block, so waiting for it here never leaves the ring empty.
+        const int aux_kb = min(w.kb0 + 2, w.kb1 - 1);
         for (int kb = w.kb0; kb < w.kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
@@ -291,6 +296,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             for (int i = 0; i < BLOCK_N / 64; ++i) tma_load_2d(sb + i * (BLOCK_K * 128), &tmap_b, &full_bar[stage], w.n0 + i * 64, kb * BLOCK_K);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (p.has_aux && kb == aux_kb) {
+            for (int g = 0; g < NUM_CONSUMERS; ++g) {
+              const int row0 = w.m0 + g * WG_ROWS;
+              const int boxes = slab_boxes(row0, w.n0, p.M, p.N);
+              uint8_t* slab = staging + g * STG_BYTES;
+              mbar_wait(&slab_empty[g], uphase);
+              mbar_arrive_expect_tx(&aux_full[g], boxes * SUB_BYTES);
+              for (int s = 0; s < boxes; ++s)
+                tma_load_2d(slab + s * SUB_BYTES, &tmap_aux, &aux_full[g], w.n0 + s * SUB_COLS, row0);
+            }
+          }
         }
       }
     }
@@ -308,16 +324,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   // 8c + 2q, +1
   const int q = lane & 3;
   const int lr = (warp & 3) * 16 + (lane >> 2);
+  const uint32_t slab = slab_base(stg, lr, q);
   const int ep = p.epilogue;
-  const bool has_aux = (ep == DPRB_EPI_BIAS_RESIDUAL || ep == DPRB_EPI_DGELU || ep == DPRB_EPI_DGELU_PRE);
 
   float acc[128];
   int stage = 0;
-  uint32_t phase = 0;
-  for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+  uint32_t phase = 0, uphase = 0;
+  for (int u = blockIdx.x; u < p.units; u += gridDim.x, uphase ^= 1) {
     const Unit w = unit_at(p, u);
     {
       int prev = -1;
+      // thread 0 hands the slab to the producer's aux load here, a full mainloop after the last unit's stores
+      const int release_kb = min(w.kb0 + 1, w.kb1 - 1);
       for (int kb = w.kb0; kb < w.kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + a_off;
@@ -330,6 +348,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         if (prev >= 0) {
           __syncwarp();
           if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        if (p.has_aux && kb == release_kb && t == 0) {
+          tma_store_wait_read();
+          mbar_arrive(&slab_empty[wg]);
         }
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -346,50 +368,53 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       case DPRB_EPI_F32_STORE: epilogue_f32<false>(p, acc, row0, w.n0, lr, q); continue;
       default: break;
     }
-    wg_bar(wg);   // the previous unit's slab_store has read the slab
-    if (has_aux) {
-      slab_load(stg, reinterpret_cast<const uint16_t*>(p.aux), p.ld_aux, row0, w.n0, p.M, p.N, t);
-      wg_bar(wg);
-    }
+    if (p.has_aux) mbar_wait(&aux_full[wg], uphase);   // the producer loaded it after the slab was released above
+    else if (t == 0) tma_store_wait_read();            // the previous unit's stores have read the slab
+    // also reconverges the warpgroup after the waits: the column-sum shuffles then need no divergence fallback
+    wg_bar(wg);
     const bool cs = p.colsum != nullptr, drop = p.drop.on();
     switch (ep) {
       case DPRB_EPI_BIAS:
-        if (cs) epilogue16<DPRB_EPI_BIAS, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
-        else epilogue16<DPRB_EPI_BIAS, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+        if (cs) epilogue16<DPRB_EPI_BIAS, false, true>(p, acc, slab, row0, w.n0, lr, q, lane);
+        else epilogue16<DPRB_EPI_BIAS, false, false>(p, acc, slab, row0, w.n0, lr, q, lane);
         break;
-      case DPRB_EPI_BIAS_GELU: epilogue16<DPRB_EPI_BIAS_GELU, false, false>(p, acc, stg, row0, w.n0, lr, q, lane); break;
+      case DPRB_EPI_BIAS_GELU: epilogue16<DPRB_EPI_BIAS_GELU, false, false>(p, acc, slab, row0, w.n0, lr, q, lane); break;
       case DPRB_EPI_BIAS_RESIDUAL:
         if (drop) {
-          if (cs) epilogue16<DPRB_EPI_BIAS_RESIDUAL, true, true>(p, acc, stg, row0, w.n0, lr, q, lane);
-          else epilogue16<DPRB_EPI_BIAS_RESIDUAL, true, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+          if (cs) epilogue16<DPRB_EPI_BIAS_RESIDUAL, true, true>(p, acc, slab, row0, w.n0, lr, q, lane);
+          else epilogue16<DPRB_EPI_BIAS_RESIDUAL, true, false>(p, acc, slab, row0, w.n0, lr, q, lane);
         } else {
-          if (cs) epilogue16<DPRB_EPI_BIAS_RESIDUAL, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
-          else epilogue16<DPRB_EPI_BIAS_RESIDUAL, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+          if (cs) epilogue16<DPRB_EPI_BIAS_RESIDUAL, false, true>(p, acc, slab, row0, w.n0, lr, q, lane);
+          else epilogue16<DPRB_EPI_BIAS_RESIDUAL, false, false>(p, acc, slab, row0, w.n0, lr, q, lane);
         }
         break;
       case DPRB_EPI_DGELU:
-        if (cs) epilogue16<DPRB_EPI_DGELU, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
-        else epilogue16<DPRB_EPI_DGELU, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+        if (cs) epilogue16<DPRB_EPI_DGELU, false, true>(p, acc, slab, row0, w.n0, lr, q, lane);
+        else epilogue16<DPRB_EPI_DGELU, false, false>(p, acc, slab, row0, w.n0, lr, q, lane);
         break;
       default:
-        if (cs) epilogue16<DPRB_EPI_DGELU_PRE, false, true>(p, acc, stg, row0, w.n0, lr, q, lane);
-        else epilogue16<DPRB_EPI_DGELU_PRE, false, false>(p, acc, stg, row0, w.n0, lr, q, lane);
+        if (cs) epilogue16<DPRB_EPI_DGELU_PRE, false, true>(p, acc, slab, row0, w.n0, lr, q, lane);
+        else epilogue16<DPRB_EPI_DGELU_PRE, false, false>(p, acc, slab, row0, w.n0, lr, q, lane);
         break;
     }
+    fence_proxy_async_smem();   // make the slab writes visible to the TMA store
     wg_bar(wg);
-    slab_store(stg, reinterpret_cast<uint16_t*>(p.D), p.ldd, row0, w.n0, p.M, p.N, t);
-    if (ep == DPRB_EPI_BIAS_GELU && p.out2 != nullptr) {
+    if (t == 0) slab_tma_store(&tmap_d, stg, row0, w.n0, p.M, p.N);
+    if (p.has_out2) {
+      // one slab for both outputs: out2 waits until D's stores have read it
+      if (t == 0) tma_store_wait_read();
       wg_bar(wg);
 #pragma unroll
       for (int c = 0; c < 32; ++c)
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-          *reinterpret_cast<uint32_t*>(stg + (lr + 8 * h) * (STG_LD * 2) + (8 * c + 2 * q) * 2) =
-              pack_bf16x2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]);
+          sts32(slab_pair(slab, c, h), pack_bf16x2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]));
+      fence_proxy_async_smem();
       wg_bar(wg);
-      slab_store(stg, reinterpret_cast<uint16_t*>(p.out2), p.ldd, row0, w.n0, p.M, p.N, t);
+      if (t == 0) slab_tma_store(&tmap_out2, stg, row0, w.n0, p.M, p.N);
     }
   }
+  if (t == 0) tma_store_wait_all();   // the slab must outlive the stores that read it
 }
 
 // ---------------------------------------------------------------- host side
@@ -451,7 +476,8 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
                "gemm: bf16 output must be 16-byte aligned with ldd %% 8 == 0 (ldd=%lld)", ldd);
   DPRB_REQUIRE(!f32_out || (ldd % 4 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0),
                "gemm: fp32 output must be 16-byte aligned with ldd %% 4 == 0 (ldd=%lld)", ldd);
-  if (epilogue == DPRB_EPI_BIAS_RESIDUAL || epilogue == DPRB_EPI_DGELU || epilogue == DPRB_EPI_DGELU_PRE)
+  const bool has_aux = epilogue == DPRB_EPI_BIAS_RESIDUAL || epilogue == DPRB_EPI_DGELU || epilogue == DPRB_EPI_DGELU_PRE;
+  if (has_aux)
     DPRB_REQUIRE(aux != nullptr && ld_aux % 8 == 0 && (reinterpret_cast<uintptr_t>(aux) & 15) == 0,
                  "gemm: epilogue %d needs a 16-byte aligned aux with ld %% 8 == 0", epilogue);
   if (bias != nullptr) DPRB_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "gemm: bias not 16B aligned");
@@ -459,12 +485,20 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   DPRB_REQUIRE(colsum == nullptr || (!f32_out && epilogue != DPRB_EPI_BIAS_GELU),
                "gemm: colsum is supported for the BIAS / BIAS_RESIDUAL / DGELU epilogues only");
 
-  CUtensorMap ta, tb;
+  const bool has_out2 = epilogue == DPRB_EPI_BIAS_GELU && out2 != nullptr;
+  if (has_out2)
+    DPRB_REQUIRE((reinterpret_cast<uintptr_t>(out2) & 15) == 0, "gemm: out2 not 16-byte aligned");
+
+  // 16-bit outputs, aux and out2 move as 64-row x 64-column boxes: one per subtile of a warpgroup's staging slab
+  CUtensorMap ta, tb, td{}, tx{}, to2{};
   int rc;
   if (!a_mn_major) rc = make_tmap(&ta, A, M, K, lda, BLOCK_M); else rc = make_tmap(&ta, A, K, M, lda, BLOCK_K);
   if (rc) return rc;
   if (!b_mn_major) rc = make_tmap(&tb, B, N, K, ldb, BLOCK_N); else rc = make_tmap(&tb, B, K, N, ldb, BLOCK_K);
   if (rc) return rc;
+  if (!f32_out && (rc = make_tmap(&td, D, M, N, ldd, WG_ROWS))) return rc;
+  if (has_aux && (rc = make_tmap(&tx, aux, M, N, ld_aux, WG_ROWS))) return rc;
+  if (has_out2 && (rc = make_tmap(&to2, out2, M, N, ldd, WG_ROWS))) return rc;
 
   GemmParams p;
   p.M = M; p.N = N; p.K = K;
@@ -479,14 +513,11 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   p.k_blocks_per_split = (p.k_blocks_total + splits - 1) / splits;
   p.splits = (p.k_blocks_total + p.k_blocks_per_split - 1) / p.k_blocks_per_split;
   p.epilogue = epilogue;
-  p.D = D; p.ldd = ldd; p.bias = bias; p.aux = reinterpret_cast<const bf16*>(aux); p.ld_aux = ld_aux;
-  p.out2 = reinterpret_cast<bf16*>(out2); p.alpha = alpha;
+  p.D = D; p.ldd = ldd; p.bias = bias; p.has_aux = has_aux; p.has_out2 = has_out2; p.alpha = alpha;
   p.colsum = colsum;
   p.aux_f16 = aux_f16; p.out_f16 = out_f16;
   p.save_pre = (dt_flags & DPRB_GEMM_SAVE_PRE) != 0;
   p.drop = drop_from_site(epilogue == DPRB_EPI_BIAS_RESIDUAL ? dropout_p : 0.f, drop_site_seed);
-  if (epilogue == DPRB_EPI_BIAS_GELU && out2 != nullptr)
-    DPRB_REQUIRE((reinterpret_cast<uintptr_t>(out2) & 15) == 0, "gemm: out2 not 16-byte aligned");
 
   p.units = tiles * p.splits;
   const int grid = p.units < sms ? p.units : sms;   // persistent: one CTA per SM
@@ -503,7 +534,7 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   auto launch = [&](auto kern) -> int {
     const bool prof = g_prof.enabled && g_prof.used + 2 <= g_prof.ev.size();
     if (prof) DPRB_CHECK_CUDA(cudaEventRecord(g_prof.ev[g_prof.used], stream));
-    kern<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p);
+    kern<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, td, tx, to2, p);
     DPRB_LAUNCH_CHECK();
     if (prof) {
       DPRB_CHECK_CUDA(cudaEventRecord(g_prof.ev[g_prof.used + 1], stream));

@@ -13,17 +13,23 @@ dev = "cuda"
 bf = torch.bfloat16
 
 
-def run(name, M, N, K, a_mn, b_mn, epi, aux=False, out2=False, colsum=False, f32=False, iters=5):
+def run(name, M, N, K, a_mn, b_mn, epi, aux=False, out2=False, colsum=False, f32=False, drop=0.0, f16=False,
+        aux_stride=1, iters=5):
+    """f16: fp16 residual in and fp16 sum out (the encoder's residual stream); drop: hidden dropout before the residual;
+    aux_stride: the aux rows are that many rows apart in a taller buffer (the pruned last layer reads CLS rows)."""
     A = torch.randn((K, M) if a_mn else (M, K), device=dev, dtype=bf)
     B = torch.randn((K, N) if b_mn else (N, K), device=dev, dtype=bf) * 0.02
-    D = torch.zeros(M, N, device=dev, dtype=torch.float32 if f32 else bf)
+    D = torch.zeros(M, N, device=dev, dtype=torch.float32 if f32 else (torch.float16 if f16 else bf))
     bias = torch.zeros(N, device=dev) if epi in (0, 1, 2) and not f32 else None
-    ax = torch.randn(M, N, device=dev, dtype=bf) if aux else None
+    ax = torch.randn(M * aux_stride, N, device=dev, dtype=torch.float16 if f16 else bf) if aux else None
     o2 = torch.empty(M, N, device=dev, dtype=bf) if out2 else None
     cs = torch.zeros(N, device=dev) if colsum else None
     lda = M if a_mn else K
     ldb = N if b_mn else K
-    f = lambda: ops.gemm(A, B, D, M, N, K, lda, ldb, N, a_mn, b_mn, epi, bias, ax, N if aux else 0, o2, 1.0, 0 if f32 else 1, cs)
+    if f16:
+        epi |= ops.GEMM_AUX_F16 | ops.GEMM_OUT_F16
+    f = lambda: ops.gemm(A, B, D, M, N, K, lda, ldb, N, a_mn, b_mn, epi, bias, ax, N * aux_stride if aux else 0, o2, 1.0,
+                         0 if f32 else 1, cs, drop, 0x5EED if drop else 0)
     Am = A.T if a_mn else A          # [M, K] views of the same storage
     Bm = B if b_mn else B.T          # [K, N]
     C = torch.empty(M, N, device=dev, dtype=bf)
@@ -53,6 +59,12 @@ run("fwd ffn-in bias only", T, I, H, 0, 0, 0)
 run("fwd ffn-in gelu (no pre)", T, I, H, 0, 0, 1)
 run("fwd ffn-in gelu + pre", T, I, H, 0, 0, 1, out2=True)
 run("fwd ffn-out bias+res", T, H, I, 0, 0, 2, aux=True)
+# what the training step runs: fp16 residual stream, hidden dropout p = 0.1
+run("fwd attn-out bias+res+drop", T, H, H, 0, 0, 2, aux=True, f16=True, drop=0.1)
+run("fwd ffn-out bias+res+drop", T, H, I, 0, 0, 2, aux=True, f16=True, drop=0.1)
+# pruned last layer: the CLS rows of T / 128 sequences, residual rows S * H apart
+run("fwd pruned attn-out res, ld_aux=S*H", T // 128, H, H, 0, 0, 2, aux=True, f16=True, drop=0.1, aux_stride=128,
+    iters=50)
 run("dgrad w2 plain", T, I, H, 0, 1, 0)
 run("dgrad w2 dgelu", T, I, H, 0, 1, 3, aux=True)
 run("dgrad w2 dgelu+colsum", T, I, H, 0, 1, 3, aux=True, colsum=True)
