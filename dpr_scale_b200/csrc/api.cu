@@ -95,6 +95,14 @@ int dprb_attn_bwd(const void* qkv, const int32_t* attn_mask, const void* ctx, co
   return attn_bwd_lse(qkv, attn_mask, ctx, lse, dctx, dqkv, dbias, nseq, Sq, heads, dropout_p, dropout_site_seed,
                       S(stream));
 }
+int dprb_attn_cls_fwd(const void* qkv, const int32_t* attn_mask, void* ctx_cls, float* probs, int nseq, int Sq,
+                      int heads, float dropout_p, uint64_t dropout_site_seed, dprb_stream_t stream) {
+  return attn_cls_fwd(qkv, attn_mask, ctx_cls, probs, nseq, Sq, heads, dropout_p, dropout_site_seed, S(stream));
+}
+int dprb_attn_cls_bwd(const void* qkv, const float* probs, const void* dctx_cls, void* dqkv, int nseq, int Sq,
+                      int heads, float dropout_p, uint64_t dropout_site_seed, dprb_stream_t stream) {
+  return attn_cls_bwd(qkv, probs, dctx_cls, dqkv, nseq, Sq, heads, dropout_p, dropout_site_seed, S(stream));
+}
 int dprb_score_ce_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
                       const int64_t* labels, float inv_temperature, float* lse, float* loss_sum, float* logits,
                       int Q, int C, int d, dprb_stream_t stream) {

@@ -275,12 +275,14 @@ ln_bwd_kernel(const bf16* __restrict__ dy, const float* __restrict__ dy_cls, int
       pf_mean = st.x; pf_rstd = st.y;
     }
     if (sparse_dy && (row % cls_stride != 0)) {
-      // upstream gradient is identically zero for this row
-      if (dz != nullptr) {
+      // upstream gradient is identically zero for this row, and so is its dropped copy (the next GEMMs read every row)
 #pragma unroll
-        for (int i = 0; i < MAXC; ++i)
-          if (act[i]) *reinterpret_cast<uint4*>(dz + (long long)row * H + (lane + 32 * i) * 8) = make_uint4(0, 0, 0, 0);
-      }
+      for (int i = 0; i < MAXC; ++i)
+        if (act[i]) {
+          const long long o = (long long)row * H + (lane + 32 * i) * 8;
+          if (dz != nullptr) *reinterpret_cast<uint4*>(dz + o) = make_uint4(0, 0, 0, 0);
+          if (dzm != nullptr) *reinterpret_cast<uint4*>(dzm + o) = make_uint4(0, 0, 0, 0);
+        }
       continue;
     }
     const float mean = dense_path ? pf_mean : stats[2 * (long long)row];

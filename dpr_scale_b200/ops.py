@@ -85,10 +85,14 @@ def ln_fwd(z, gamma, beta, eps, cls_stride=0, y_res=None):
     return y, stats, cls
 
 
-def ln_bwd(dy, z, stats, gamma, dgamma, dbeta, dbias=None, dy_cls=None, cls_stride=1, dropout_p=0.0, site_seed=0):
+def ln_bwd(dy, z, stats, gamma, dgamma, dbeta, dbias=None, dy_cls=None, cls_stride=1, dropout_p=0.0, site_seed=0,
+           dz=None, dzm=None):
+    """dz / dzm: optional preallocated bf16 [T, H] outputs."""
     T, H = z.shape
-    dz = torch.empty(z.shape, dtype=torch.bfloat16, device=z.device)      # gradients are bf16 whatever z holds
-    dzm = torch.empty_like(dz) if dropout_p > 0 else None
+    if dz is None:
+        dz = torch.empty(z.shape, dtype=torch.bfloat16, device=z.device)      # gradients are bf16 whatever z holds
+    if dzm is None and dropout_p > 0:
+        dzm = torch.empty_like(dz)
     check(_lib.load().dprb_ln_bwd(_ptr(dy), _ptr(dy_cls), cls_stride, _ptr(z), _ptr(stats), _ptr(gamma), _ptr(dz),
                                   _ptr(dgamma), _ptr(dbeta), _ptr(dbias), T, H, _ptr(dzm), float(dropout_p),
                                   int(site_seed), int(z.dtype == torch.float16), _stream()), "dprb_ln_bwd")
@@ -134,6 +138,25 @@ def attn_bwd(qkv, attn_mask, ctx, lse, dctx, nseq, S, heads, dbias=None, dropout
     check(_lib.load().dprb_attn_bwd(_ptr(qkv), _ptr(attn_mask), _ptr(ctx), _ptr(lse), _ptr(dctx), _ptr(dqkv),
                                     _ptr(dbias), nseq, S, heads, float(dropout_p), int(site_seed), _stream()),
           "dprb_attn_bwd")
+    return dqkv
+
+
+def attn_cls_fwd(qkv, attn_mask, nseq, S, heads, dropout_p=0.0, site_seed=0):
+    """Single-query attention of the pruned last layer (test hook): (ctx_cls bf16 [nseq, H], probs fp32 [nseq, heads, S])."""
+    H = heads * 64
+    ctx = torch.empty(nseq, H, dtype=torch.bfloat16, device=qkv.device)
+    probs = torch.empty(nseq, heads, S, dtype=torch.float32, device=qkv.device)
+    check(_lib.load().dprb_attn_cls_fwd(_ptr(qkv), _ptr(attn_mask), _ptr(ctx), _ptr(probs), nseq, S, heads,
+                                        float(dropout_p), int(site_seed), _stream()), "dprb_attn_cls_fwd")
+    return ctx, probs
+
+
+def attn_cls_bwd(qkv, probs, dctx_cls, nseq, S, heads, dropout_p=0.0, site_seed=0, dqkv=None):
+    """dqkv bf16 [nseq*S, 3H], every element written (dqkv: optional preallocated output)."""
+    if dqkv is None:
+        dqkv = torch.empty_like(qkv)
+    check(_lib.load().dprb_attn_cls_bwd(_ptr(qkv), _ptr(probs), _ptr(dctx_cls), _ptr(dqkv), nseq, S, heads,
+                                        float(dropout_p), int(site_seed), _stream()), "dprb_attn_cls_bwd")
     return dqkv
 
 

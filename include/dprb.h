@@ -150,6 +150,17 @@ int dprb_attn_fwd(const void* qkv_bf16, const int32_t* attn_mask, void* ctx_bf16
 int dprb_attn_bwd(const void* qkv_bf16, const int32_t* attn_mask, const void* ctx_bf16, const float* lse,
                   const void* dctx_bf16, void* dqkv_bf16, float* dbias, int nseq, int S, int heads,
                   float dropout_p, uint64_t dropout_site_seed, dprb_stream_t stream);
+/* Single-query (CLS row) attention of the encoder's pruned last layer, where only query 0 of each sequence attends
+ * (test hooks: the encoder calls these kernels internally).  Same qkv / attn_mask layout and dropout site as
+ * dprb_attn_fwd; the probability dropout of query 0 of problem (seq, h) uses row (seq*heads + h)*S of site 1.
+ *   ctx_cls: bf16 [nseq, H]  = softmax(q_0 K^T / 8 + key_mask) V per head;
+ *   probs:   fp32 [nseq, heads, S] the (undropped) probabilities of query 0, written by fwd and read by bwd;
+ *   dqkv:    bf16 [nseq*S, 3H] fully written by bwd: dQ on row 0 of each sequence (zeros on rows 1..S-1), dK / dV on
+ *            every row (zeros for masked keys). */
+int dprb_attn_cls_fwd(const void* qkv_bf16, const int32_t* attn_mask, void* ctx_cls_bf16, float* probs, int nseq, int S,
+                      int heads, float dropout_p, uint64_t dropout_site_seed, dprb_stream_t stream);
+int dprb_attn_cls_bwd(const void* qkv_bf16, const float* probs, const void* dctx_cls_bf16, void* dqkv_bf16, int nseq,
+                      int S, int heads, float dropout_p, uint64_t dropout_site_seed, dprb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Fused in-batch-negative scoring + softmax cross-entropy.

@@ -199,8 +199,16 @@ def check_ln(T=777, H=768, cls_stride=0, seed=1, f16=False):
     return res
 
 
-def check_embed(T=500, H=768, vocab=1000, max_pos=64, type_vocab=2, seed=2):
+def check_embed(T=500, H=768, vocab=1000, max_pos=64, type_vocab=2, seed=2, dropout=0.0, y_res=False, roberta_S=0):
+    """dropout: embedding dropout (site 0 of layer 0), replayed from dprb_dropout_mask(T, H, p, seed, 0, 0);
+    y_res: the fp16 residual-stream copy of the output; type_vocab >= 3 takes the per-element atomic branch of the
+    type-table gradient; roberta_S: RoBERTa's pad-derived positions (cumsum of non-pad tokens + pad id) over sequences
+    of roberta_S tokens, so the position changes between the rows one warp handles (T above the 4224 warps of the
+    grid gives every warp several rows)."""
     g = torch.Generator().manual_seed(seed)
+    if roberta_S:
+        pad = 1
+        max_pos = roberta_S + pad + 1
     word = torch.randn(vocab, H, generator=g) * 0.5
     pos = torch.randn(max_pos, H, generator=g) * 0.5
     typ = torch.randn(type_vocab, H, generator=g) * 0.5
@@ -209,19 +217,36 @@ def check_embed(T=500, H=768, vocab=1000, max_pos=64, type_vocab=2, seed=2):
     ids = torch.randint(0, vocab, (T,), generator=g)
     ids[:50] = 7  # repeated ids -> atomic accumulation
     tts = torch.randint(0, type_vocab, (T,), generator=g)
-    pids = torch.arange(T) % max_pos
+    if roberta_S:
+        assert T % roberta_S == 0
+        ids = torch.randint(2, vocab, (T // roberta_S, roberta_S), generator=g)
+        lens = torch.randint(1, roberta_S + 1, (T // roberta_S,), generator=g)
+        ids[torch.arange(roberta_S).unsqueeze(0) >= lens.unsqueeze(1)] = pad
+        pids = oenc.roberta_position_ids(ids, pad).flatten()
+        ids = ids.flatten()
+    else:
+        pids = torch.arange(T) % max_pos
     eps = 1e-12
     res = {}
     d = lambda t: t.to(DEV)
-    y, stats = ops.embed_ln_fwd(d(ids), d(tts), d(pids), d(word), d(pos), d(typ), d(gamma), d(beta), eps)
+    dseed = 0xE3B + seed
+    yres = torch.empty(T, H, dtype=torch.float16, device=DEV) if y_res else None
+    y, stats = ops.embed_ln_fwd(d(ids), d(tts), d(pids), d(word), d(pos), d(typ), d(gamma), d(beta), eps, dropout, dseed,
+                                yres)
     wr, pr, tr = (t.clone().requires_grad_(True) for t in (word, pos, typ))
     gr, br = gamma.clone().requires_grad_(True), beta.clone().requires_grad_(True)
     yr = oenc.layer_norm((wr[ids] + tr[tts]) + pr[pids], gr, br, eps)
+    if dropout:
+        keep = ops.dropout_mask(T, H, dropout, dseed, 0, 0).float().cpu()
+        yr = yr * keep / (1.0 - round(dropout * 65536) / 65536.0)
     _close("emb_y", y, yr, 2 ** -7, 1e-3, res)
+    if y_res:
+        _close("emb_y_res", yres, yr, 2 ** -10, 1e-3, res)
     dy = _bf(torch.randn(T, H, generator=g))
     dword, dpos, dtyp = torch.zeros_like(d(word)), torch.zeros_like(d(pos)), torch.zeros_like(d(typ))
     dgamma, dbeta = torch.zeros(H, device=DEV), torch.zeros(H, device=DEV)
-    ops.embed_ln_bwd(d(dy), d(ids), d(tts), d(pids), d(word), d(pos), d(typ), d(gamma), stats, dword, dpos, dtyp, dgamma, dbeta)
+    ops.embed_ln_bwd(d(dy), d(ids), d(tts), d(pids), d(word), d(pos), d(typ), d(gamma), stats, dword, dpos, dtyp, dgamma,
+                     dbeta, dropout, dseed)
     yr.backward(dy.float())
     _close("emb_dword", dword, wr.grad, 1e-4, 1e-3, res)
     _close("emb_dpos", dpos, pr.grad, 1e-4, 1e-3, res)
@@ -406,6 +431,27 @@ CHECKS["attn_tc2_s200"] = lambda: check_attention(3, 200, 2, True, seed=12)
 CHECKS["attn_tc2_s256_many"] = lambda: check_attention(20, 256, 4, True, seed=13)
 CHECKS["attn_tc_drop_s128"] = lambda: check_attention(4, 128, 2, True, seed=14, dropout=0.1)
 CHECKS["attn_tc2_drop_s200"] = lambda: check_attention(3, 200, 2, True, seed=15, dropout=0.1)
+# 16 heads (H = 1024): the short (S <= 256) and key-blocked (S > 256) kernels
+CHECKS["attn_h16_s128"] = lambda: check_attention(2, 128, 16, True, seed=80)
+CHECKS["attn_h16_s256"] = lambda: check_attention(2, 256, 16, True, seed=81)
+CHECKS["attn_h16_s512"] = lambda: check_attention(2, 512, 16, True, seed=82)
+CHECKS["attn_h16_drop_s200"] = lambda: check_attention(2, 200, 16, True, seed=83, dropout=0.1)
+
+# LayerNorm widths: H = 256 / 512 take the paired-column kernels at MAXC 1 / 2; H = 320 / 640 / 896 the generic kernels
+# with a partly active last chunk (MAXC 2 / 3 / 4).  Each with and without the fp16 stream and the CLS-row output.
+for _H in (256, 320, 512, 640, 896):
+    CHECKS[f"ln_{_H}"] = lambda H=_H: check_ln(777, H, seed=H)
+    CHECKS[f"ln_{_H}_f16"] = lambda H=_H: check_ln(777, H, seed=H + 1, f16=True)
+    CHECKS[f"ln_{_H}_cls"] = lambda H=_H: check_ln(640, H, cls_stride=40, seed=H + 2)
+    CHECKS[f"ln_{_H}_cls_f16"] = lambda H=_H: check_ln(640, H, cls_stride=40, seed=H + 3, f16=True)
+
+# embeddings: dropout, the fp16 y_res copy, one and three token types, RoBERTa positions; T = 9000 rows (> 4224 warps)
+for _H in (256, 320, 768, 1024):
+    CHECKS[f"embed_{_H}_drop_yres_tt3"] = lambda H=_H: check_embed(9000, H, type_vocab=3, seed=H, dropout=0.1,
+                                                                   y_res=True)
+    CHECKS[f"embed_{_H}_roberta_tt1"] = lambda H=_H: check_embed(9000, H, type_vocab=1, seed=H + 1, y_res=True,
+                                                                 dropout=0.1 if H in (320, 1024) else 0.0,
+                                                                 roberta_S=100)
 
 
 # ------------------------------------------------------------------ retrieval
