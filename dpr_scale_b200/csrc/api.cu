@@ -156,6 +156,10 @@ int dprb_encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b,
                      int layer_lo, int layer_hi, dprb_stream_t stream) {
   return encoder_bwd(w, b, dpooled, layer_lo, layer_hi, S(stream));
 }
+int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
+                         int H, int L, dprb_stream_t stream) {
+  return seqcls_head_fwd(pre, weight, bias, logits, score, N, H, L, S(stream));
+}
 int64_t dprb_search_workspace_bytes(int64_t Q, int k) { return search_workspace_bytes(Q, k); }
 int dprb_search_topk(const void* queries, const void* corpus, int dtype, int64_t Q, int64_t N, int d, int k,
                      int64_t index_offset, float* out_scores, int64_t* out_index, void* workspace,

@@ -102,6 +102,9 @@ long long topk_merge_workspace_bytes(long long Q, int total);
 int topk_merge(const float* scores, const long long* index, long long Q, int total, int k, float* out_scores,
                long long* out_index, void* workspace, long long workspace_bytes, cudaStream_t stream);
 
+int seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
+                    int H, int L, cudaStream_t stream);
+
 long long encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S, int save);
 int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, cudaStream_t stream);
 int encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, const float* dpooled, int layer_lo,

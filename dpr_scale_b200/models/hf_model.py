@@ -275,16 +275,18 @@ class _WorkspacePool:
 class _Transformer(nn.Module):
     """Container that owns the arenas and mirrors the HF module tree (parameter names only)."""
 
-    def __init__(self, cfg, master: torch.Tensor):
+    def __init__(self, cfg, master: torch.Tensor, pooler: bool = True):
         super().__init__()
         self.cfg = cfg
         self.layout = ParamLayout(cfg)
         assert master.numel() == self.layout.total
         self._bind(master)
         H = cfg["hidden_size"]
-        # HF's pooler is part of the reference state_dict but never used (hf_model.py:39) and gets no grad.
-        self.add_module("pooler", nn.Module())
-        self.pooler.add_module("dense", nn.Linear(H, H))
+        # HF's pooler is part of the reference state_dict but never used (hf_model.py:39) and gets no grad.  A BERT
+        # cross-encoder uses it as the first layer of its classification head; RoBERTa's has none (pooler=False).
+        if pooler:
+            self.add_module("pooler", nn.Module())
+            self.pooler.add_module("dense", nn.Linear(H, H))
         # Checkpoints written with the reference's pinned transformers==3.4.0 carry the persistent buffer
         # `embeddings.position_ids` (later releases made it non-persistent); it holds arange(max_pos) and is not a
         # weight, so it is dropped on load instead of failing a strict load_state_dict.
@@ -309,7 +311,8 @@ class _Transformer(nn.Module):
         master = fn(self._master)
         if master.dtype != torch.float32:
             raise TypeError("dprb encoder master weights must stay fp32 (bf16 shadows are managed internally)")
-        self.pooler._apply(fn)
+        if "pooler" in self._modules:
+            self.pooler._apply(fn)
         self._bind(master)
         return self
 
@@ -323,9 +326,13 @@ class _Transformer(nn.Module):
 
 class HFEncoder(nn.Module):
     def __init__(self, model_path: str = "roberta-base", dropout: float = 0.1,
-                 projection_dim: Optional[int] = None, _config=None, _seed: Optional[int] = None):
+                 projection_dim: Optional[int] = None, _config=None, _seed: Optional[int] = None, _state=None,
+                 _pooler: bool = True):
         super().__init__()
-        if _config is not None:
+        if _config is not None and _state is not None:     # config + HF state dict already read by the caller
+            cfg, sd = _normalise_config(_config), _state
+            master = torch.zeros(ParamLayout(cfg).total, dtype=torch.float32)
+        elif _config is not None:
             cfg = _normalise_config(_config)
             master = self._random_init(cfg, _seed if _seed is not None else 0)
             sd = None
@@ -334,7 +341,7 @@ class HFEncoder(nn.Module):
             master = torch.zeros(ParamLayout(cfg).total, dtype=torch.float32)
         self.config = cfg
         self.dropout = float(dropout)
-        self.transformer = _Transformer(cfg, master)
+        self.transformer = _Transformer(cfg, master, pooler=_pooler)
         if sd is not None:
             self._load_hf_state(sd)
         self.project = nn.Identity()

@@ -268,6 +268,21 @@ def cast_bf16_f32(src, dst):
     return dst
 
 
+SEQCLS_MAX_LABELS = 16   # include/dprb.h DPRB_SEQCLS_MAX_LABELS
+
+
+def seqcls_head_fwd(pre, weight, bias=None):
+    """Cross-encoder classification head after its dense layer: pre fp32 [N, H], weight fp32 [L, H], bias fp32 [L]
+    -> (logits fp32 [N, L] = tanh(pre) @ weight.T + bias, score fp32 [N] = max over labels)."""
+    N, H = pre.shape
+    L = weight.shape[0]
+    logits = torch.empty(N, L, dtype=torch.float32, device=pre.device)
+    score = torch.empty(N, dtype=torch.float32, device=pre.device)
+    check(_lib.load().dprb_seqcls_head_fwd(_ptr(pre), _ptr(weight), _ptr(bias), _ptr(logits), _ptr(score), N, H, L,
+                                           _stream()), "dprb_seqcls_head_fwd")
+    return logits, score
+
+
 _SEARCH_WS = {}
 
 

@@ -272,6 +272,24 @@ int dprb_encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b,
                      int layer_lo, int layer_hi, dprb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Cross-encoder sequence-classification head (reranking: dpr_scale/models/citadel_models/cross_encoder.py:21-26,
+ * AutoModelForSequenceClassification under no_grad).  The caller runs the head's dense layer first, on the CLS rows
+ * that dprb_encoder_fwd returns: dprb_gemm_bf16 with DPRB_EPI_F32_STORE (bf16 operands, fp32 accumulate + bias) gives
+ * pre fp32 [N, H].  This entry point does the rest in fp32:
+ *   logits[n, l] = tanh(pre[n, :]) . weight[l, :] + bias[l]      (bias may be NULL)
+ *   score[n]     = max_l logits[n, l]                             (optional: score may be NULL)
+ * It replaces, in site-packages/transformers:
+ *   BERT: BertPooler.forward (models/bert/modeling_bert.py: dense -> tanh on token 0) and the dropout + classifier
+ *         Linear of BertForSequenceClassification.forward (dropout is the identity in eval);
+ *   RoBERTa / XLM-R: RobertaClassificationHead.forward (models/roberta/modeling_roberta.py: token 0 -> dense -> tanh
+ *         -> out_proj).
+ * pre and weight fp32 row-major, 16-byte aligned; requires H % 8 == 0, H <= 1024, 1 <= L <= DPRB_SEQCLS_MAX_LABELS
+ * (checked before any launch, return code 1). */
+#define DPRB_SEQCLS_MAX_LABELS 16
+int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
+                         int H, int L, dprb_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Brute-force retrieval : replaces search_index() of
  * dpr_scale/run_retrieval_pytorch.py:141-176 -- einsum('ik,jk->ij') in fp16 followed by torch.topk over the
  * materialised [Q, N] score matrix -- with one fused pass: the corpus is streamed once per block of 128 queries
