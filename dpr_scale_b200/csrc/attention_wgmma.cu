@@ -45,8 +45,10 @@ attn_fwd_wg_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   uint64_t* bar = reinterpret_cast<uint64_t*>(sMask + NK);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, q4 = lane & 3;
-  const int prob = blockIdx.y, seq = prob / heads, h = prob - seq * heads;
-  const int qb = blockIdx.x;
+  // 1-D grid, query blocks of one problem adjacent: gridDim.y (65 535) would cap nseq * heads
+  const int nqb = (S + 63) / 64;
+  const int prob = blockIdx.x / nqb, qb = blockIdx.x - prob * nqb;
+  const int seq = prob / heads, h = prob - seq * heads;
   const int H = heads * 64;
   if (tid == 0) {
     tma_prefetch_desc(&tm_q);
@@ -360,9 +362,10 @@ int fwd_launch(const CUtensorMap& tq, const CUtensorMap& tkv, const int32_t* att
     DPRB_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_wg_kernel<NK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr = true;
   }
-  const dim3 grid((S + 63) / 64, nseq * heads);
-  if (drop.on()) attn_fwd_wg_kernel<NK, true><<<grid, 128, smem, stream>>>(tq, tkv, attn_mask, (bf16*)ctx, lse, S, heads, drop);
-  else attn_fwd_wg_kernel<NK, false><<<grid, 128, smem, stream>>>(tq, tkv, attn_mask, (bf16*)ctx, lse, S, heads, drop);
+  const long long grid = (long long)((S + 63) / 64) * nseq * heads;
+  DPRB_REQUIRE(grid < (1LL << 31), "attn_fwd: grid too large");
+  if (drop.on()) attn_fwd_wg_kernel<NK, true><<<(unsigned)grid, 128, smem, stream>>>(tq, tkv, attn_mask, (bf16*)ctx, lse, S, heads, drop);
+  else attn_fwd_wg_kernel<NK, false><<<(unsigned)grid, 128, smem, stream>>>(tq, tkv, attn_mask, (bf16*)ctx, lse, S, heads, drop);
   DPRB_LAUNCH_CHECK();
   return 0;
 }

@@ -123,18 +123,24 @@ def colsum(x, out):
     return out
 
 
-def attn_fwd(qkv, attn_mask, nseq, S, heads, need_lse=True, dropout_p=0.0, site_seed=0):
+def attn_fwd(qkv, attn_mask, nseq, S, heads, need_lse=True, dropout_p=0.0, site_seed=0, ctx=None, lse=None):
+    """ctx bf16 [nseq*S, H], lse fp32 [nseq, heads, S] (ctx / lse: optional preallocated outputs; the kernels write
+    the first nseq*S rows and nseq*heads*S values)."""
     T = nseq * S
     H = heads * 64
-    ctx = torch.empty(T, H, dtype=torch.bfloat16, device=qkv.device)
-    lse = torch.empty(nseq, heads, S, dtype=torch.float32, device=qkv.device) if need_lse else None
+    if ctx is None:
+        ctx = torch.empty(T, H, dtype=torch.bfloat16, device=qkv.device)
+    if lse is None and need_lse:
+        lse = torch.empty(nseq, heads, S, dtype=torch.float32, device=qkv.device)
     check(_lib.load().dprb_attn_fwd(_ptr(qkv), _ptr(attn_mask), _ptr(ctx), _ptr(lse), nseq, S, heads, float(dropout_p),
                                     int(site_seed), _stream()), "dprb_attn_fwd")
     return ctx, lse
 
 
-def attn_bwd(qkv, attn_mask, ctx, lse, dctx, nseq, S, heads, dbias=None, dropout_p=0.0, site_seed=0):
-    dqkv = torch.empty_like(qkv)
+def attn_bwd(qkv, attn_mask, ctx, lse, dctx, nseq, S, heads, dbias=None, dropout_p=0.0, site_seed=0, dqkv=None):
+    """dqkv bf16 [nseq*S, 3H] (dqkv: optional preallocated output; the first nseq*S rows are written)."""
+    if dqkv is None:
+        dqkv = torch.empty_like(qkv)
     check(_lib.load().dprb_attn_bwd(_ptr(qkv), _ptr(attn_mask), _ptr(ctx), _ptr(lse), _ptr(dctx), _ptr(dqkv),
                                     _ptr(dbias), nseq, S, heads, float(dropout_p), int(site_seed), _stream()),
           "dprb_attn_bwd")

@@ -267,44 +267,213 @@ def check_colsum(T=1000, N=2304, seed=3):
 
 
 # ------------------------------------------------------------------ attention
-def check_attention(nseq=3, S=128, heads=2, masked=True, seed=4, dropout=0.0):
-    g = torch.Generator().manual_seed(seed)
-    H = heads * 64
-    T = nseq * S
-    qkv = _bf(torch.randn(T, 3 * H, generator=g))
+ATTN_GUARD = 64          # guard rows (ctx, dqkv) / values per head (lse) past the outputs
+
+
+def _sentinel(shape, dtype=torch.bfloat16):
+    """Buffer of all-ones bits (a NaN in bf16 and fp32): an element the kernel does not write stays non-finite."""
+    it = torch.int16 if dtype == torch.bfloat16 else torch.int32
+    return torch.full(shape, -1, dtype=it, device=DEV).view(dtype)
+
+
+def _bits(t):
+    return t.view(torch.int16 if t.dtype == torch.bfloat16 else torch.int32)
+
+
+def attn_mask(kind, nseq, S, g):
+    """int32 [nseq, S] key mask (None for "none"); every sequence keeps at least one valid key.
+      random_prefix: a valid prefix of random length in [S/4, S];
+      prefix: lengths 1, S - 1, S, and one key into the last 64- and the last 128-key block, in turn;
+      holes:  ~70 % random keys and a 20-key interior hole across a 128- (short S: a 64-) key boundary, key 0 kept;
+      left:   left padding: the first S/2 keys masked, or (S > 256) exactly the first 128-key block, in turn;
+      last:   a single valid key, at position S - 1."""
+    if kind == "none":
+        return None
     am = torch.ones(nseq, S, dtype=torch.int32)
-    if masked:
+    if kind == "random_prefix":
         for i in range(nseq):
-            ln = int(torch.randint(max(1, S // 4), S + 1, (1,), generator=g))
-            am[i, ln:] = 0
-    res = {}
-    dseed, site = 0x1234567, 0
-    keepm = None
-    if dropout > 0:  # attention-probability dropout: export the (never stored) mask and replay it in the oracle
+            am[i, int(torch.randint(max(1, S // 4), S + 1, (1,), generator=g)):] = 0
+    elif kind == "prefix":
+        lens = [1, max(1, S - 1), S, 64 * ((S - 1) // 64) + 1, 128 * ((S - 1) // 128) + 1]
+        for i in range(nseq):
+            am[i, lens[i % len(lens)]:] = 0
+    elif kind == "holes":
+        am = (torch.rand(nseq, S, generator=g) < 0.7).to(torch.int32)
+        if S >= 148:
+            am[:, 118:138] = 0
+        elif S >= 84:
+            am[:, 54:74] = 0
+        am[:, 0] = 1
+    elif kind == "left":
+        n0 = [S // 2] + ([128] if S > 256 else [])
+        for i in range(nseq):
+            am[i, :n0[i % len(n0)]] = 0
+    elif kind == "last":
+        am[:, :S - 1] = 0
+    else:
+        raise ValueError(kind)
+    return am
+
+
+def _attn_qkv(nseq, S, heads, qscale, late_max, g):
+    """bf16 [nseq*S, 3H] on the device.  qscale multiplies Q: |q.k| / 8 ~ qscale * N(0, 1), up to ~30 at qscale 10.
+    late_max: every logit is ~10 * key / S plus noise of ~0.5, so each key block raises every row's running maximum
+    (the long forward rescales O and l at every block) and the largest logit of every row sits in the last block."""
+    H = heads * 64
+    x = torch.randn(nseq * S, 3, heads, 64, device=DEV, generator=g)
+    x[:, 0] *= qscale
+    if late_max:
+        u = torch.full((64,), 0.125, device=DEV)          # unit vector shared by every query and key
+        pos = (torch.arange(nseq * S, device=DEV) % S).float() / S
+        x[:, 0] = 0.3 * x[:, 0] + 8 * u
+        x[:, 1] = 0.3 * x[:, 1] + 10 * pos[:, None, None] * u
+    return x.view(nseq * S, 3 * H).to(torch.bfloat16)
+
+
+def _per_problem(name, got, ref, rtol, atol, out, bound=None):
+    """got / ref [n, heads, rows, cols]: max |got - ref| (less `bound`, elementwise) of every (sequence, head) problem
+    against rtol * that problem's max|ref| + atol; keeps the worst problem of `name` in out."""
+    assert torch.isfinite(got).all(), f"{name}: unwritten or non-finite values"
+    err = (got - ref).abs()
+    e, sc = err.amax(dim=(-2, -1)).flatten(), ref.abs().amax(dim=(-2, -1)).flatten()
+    if bound is not None:   # the worst problem by the plain gate as well, for the record
+        out[name + "_plain"] = max(out.get(name + "_plain", 0.0), float((e / (rtol * sc + atol)).max()))
+        err = (err - bound).clamp_min(0)
+        e = err.amax(dim=(-2, -1)).flatten()
+    ratio = e / (rtol * sc + atol)
+    i = int(ratio.argmax())
+    if float(ratio[i]) >= out.get(name + "_ratio", -1.0):
+        out[name + "_ratio"], out[name + "_err"], out[name + "_scale"] = float(ratio[i]), float(e[i]), float(sc[i])
+
+
+def check_attention(nseq=3, S=128, heads=2, masked=True, seed=4, dropout=0.0, mask=None, qscale=1.0, late_max=False):
+    """dprb_attn_fwd / _bwd against a float64 softmax attention of the same bf16 qkv, computed on the device a chunk of
+    sequences at a time.  mask: a kind of attn_mask() (default: "random_prefix" if masked, else "none").
+
+    Gates, per (sequence, head) problem against that problem's max|ref|; the worst problem of each is returned as
+    <name>_err / _scale / _ratio (err over gate):
+      ctx 2^-7 * max + 1e-4 (P is rounded to bf16 before P V, ctx once more);  lse 1e-4 absolute per row;
+      dV 2^-6 * max + 1e-5 (P rounded to bf16);  dQ, dK 2^-6 * max + 1e-5 beyond a first-order bound of the error that
+      dS = P (dP - D) / 8 inherits from its inputs, elementwise, E_dQ = A |K| and E_dK = A^T |Q| with
+      A = P (2^-12 (|dP| + sum_j P |dP|) + dD) / 8: 2^-12 is the relative error of the kernel's P that the lse gate
+      allows (1e-4 = 2^-13.3, plus logit rounding), and dD = sum_d |dO| |ctx - ctx_ref| is the error of D =
+      rowsum(dO * ctx) that the long backward (S > 256) takes from the bf16 ctx (0 for S <= 256, which rebuilds D from
+      P and dP).  Without it dS = 0 rows (one valid key, or a peaked softmax at qscale 10 in the long kernels) would be
+      gated on rounding noise alone;
+      dbias (fused QKV bias gradient, accumulated into ones) 1e-5 * max|ref| against the column sums of dqkv.
+    And exactly: ctx / lse / dqkv start as a NaN sentinel with ATTN_GUARD guard rows (values) past nseq*S: every
+    element in range is written and finite, every guard element keeps its bits; dK / dV of masked keys are 0; K / V of
+    masked keys times 100 leave ctx and lse unchanged; replacing the qkv, mask and dctx of the odd sequences leaves the
+    even sequences' ctx and lse unchanged (an all-ones mask there stands in for no mask); both forwards and the long
+    backward are bitwise repeatable.  The S <= 256 backward adds dQ with shared-memory atomics from two warpgroups:
+    its repeatability is returned as bwd_repeatable, not gated.
+
+    Not covered: a sequence with no valid key (no tokenizer path produces one).  From the code the forward gives ctx 0
+    and lse -inf there and the backward NaN (exp2(-inf - -inf)), which the fused dbias spreads to every column."""
+    kind = mask if mask is not None else ("random_prefix" if masked else "none")
+    g = torch.Generator().manual_seed(seed)
+    gd = torch.Generator(device=DEV).manual_seed(seed)
+    H, T, G = heads * 64, nseq * S, ATTN_GUARD
+    qkv = _attn_qkv(nseq, S, heads, qscale, late_max, gd)
+    am = attn_mask(kind, nseq, S, g)
+    amd = am.to(DEV) if am is not None else None
+    dctx = torch.randn(T, H, device=DEV, generator=gd).to(torch.bfloat16)
+    dseed, site, keep = 0x1234567 + seed, 0, None
+    if dropout > 0:  # attention-probability dropout: export the (never stored) mask and replay it in the reference
         site = ops.dropout_site_seed(dseed, 3, 1)
-        keepm = ops.dropout_mask(nseq * heads * S, S, dropout, dseed, 3, 1).view(nseq, heads, S, S).float().cpu()
-        keepm = keepm / (1.0 - round(dropout * 65536) / 65536.0)
-    ctx, lse = ops.attn_fwd(qkv.to(DEV), am.to(DEV) if masked else None, nseq, S, heads, True, dropout, site)
-    qr = qkv.float().requires_grad_(True)
-    x = qr.view(nseq, S, 3, heads, 64)
-    q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))  # nseq, heads, S, 64
-    sc = q @ k.transpose(-1, -2) / 8.0
-    if masked:
-        sc = sc.masked_fill(am.view(nseq, 1, 1, S) == 0, float("-inf"))
-    p = torch.softmax(sc, -1)
-    if keepm is not None:
-        p = p * keepm
-    cr = (p @ v).transpose(1, 2).reshape(T, H)
-    _close("attn_ctx", ctx, cr, 2 ** -7, 2e-3, res)
-    _close("attn_lse", lse, torch.logsumexp(sc, -1), 1e-4, 1e-3, res)
-    dctx = _bf(torch.randn(T, H, generator=g))
+        keep = ops.dropout_mask(nseq * heads * S, S, dropout, dseed, 3, 1).view(nseq, heads, S, S)
+
+    def fwd(x, m):
+        cb, lb = _sentinel((T + G, H)), _sentinel((nseq * heads * S + G,), torch.float32)
+        ops.attn_fwd(x, m, nseq, S, heads, True, dropout, site, ctx=cb[:T], lse=lb[:T * heads].view(nseq, heads, S))
+        return cb, lb
+
+    def bwd(dbias):
+        db = _sentinel((T + G, 3 * H))
+        ops.attn_bwd(qkv, amd, ctx, lse, dctx, nseq, S, heads, dbias, dropout, site, dqkv=db[:T])
+        return db
+
+    ctx_b, lse_b = fwd(qkv, amd)
+    ctx, lse = ctx_b[:T], lse_b[:T * heads].view(nseq, heads, S)
     dbias = torch.ones(3 * H, device=DEV)
-    dqkv = ops.attn_bwd(qkv.to(DEV), am.to(DEV) if masked else None, ctx, lse, dctx.to(DEV), nseq, S, heads, dbias,
-                        dropout, site)
-    cr.backward(dctx.float())
-    # P and dS are rounded to bf16 before the second matmuls (as in any flash-style kernel): 2^-6 headroom
-    _close("attn_dqkv", dqkv, qr.grad, 2 ** -6, 4e-3, res)
-    _close("attn_dbias", dbias, 1 + dqkv.double().cpu().sum(0), 1e-4, 1e-3, res)  # fused QKV bias gradient
+    dqkv_b = bwd(dbias)
+    dqkv = dqkv_b[:T]
+    res = {}
+
+    # exact properties
+    ctx_b2, lse_b2 = fwd(qkv, amd)
+    assert torch.equal(_bits(ctx_b2), _bits(ctx_b)) and torch.equal(_bits(lse_b2), _bits(lse_b)), \
+        "attn_fwd is not bitwise repeatable"
+    del ctx_b2, lse_b2
+    dqkv_b2 = bwd(None)
+    res["bwd_repeatable"] = float(torch.equal(_bits(dqkv_b2), _bits(dqkv_b)))
+    assert S <= 256 or res["bwd_repeatable"], "the S > 256 attn_bwd is not bitwise repeatable"
+    del dqkv_b2
+    for name, buf in (("ctx", ctx_b[T:]), ("lse", lse_b[T * heads:]), ("dqkv", dqkv_b[T:])):
+        assert bool((_bits(buf) == -1).all()), f"{name}: written past nseq * S"
+    assert torch.isfinite(lse).all(), "lse: unwritten or non-finite values"
+    if am is not None and bool((am == 0).any()):
+        off = (amd == 0).flatten()
+        assert float(dqkv[off, H:].float().abs().max()) == 0.0, "dK / dV of masked keys must be exactly zero"
+        big = qkv.clone()
+        big[off, H:] = (big[off, H:].float() * 100).to(torch.bfloat16)
+        cb, lb = fwd(big, amd)
+        assert torch.equal(_bits(cb), _bits(ctx_b)) and torch.equal(_bits(lb), _bits(lse_b)), \
+            "K / V of masked keys changed ctx or lse"
+        del big, cb, lb
+    if nseq > 1:
+        odd = (torch.arange(T, device=DEV) // S) % 2 == 1
+        other = qkv.clone()
+        other[odd] = torch.randn(int(odd.sum()), 3 * H, device=DEV, generator=gd).to(torch.bfloat16) * 3
+        am2 = amd.clone() if amd is not None else torch.ones(nseq, S, dtype=torch.int32, device=DEV)
+        am2[1::2] = attn_mask("holes", nseq, S, g).to(DEV)[1::2]
+        cb, lb = fwd(other, am2)
+        ev = ~odd
+        assert torch.equal(_bits(cb[:T][ev]), _bits(ctx[ev])), "ctx depends on other sequences"
+        assert torch.equal(_bits(lb[:T * heads].view(nseq, heads, S)[0::2]), _bits(lse[0::2])), \
+            "lse depends on other sequences"
+        del other, am2, cb, lb
+
+    # float64 reference, a chunk of sequences at a time (at most 2^23 attention probabilities per chunk)
+    step = max(1, (1 << 23) // (heads * S * S))
+    for s0 in range(0, nseq, step):
+        s1 = min(nseq, s0 + step)
+        n, r0, r1 = s1 - s0, s0 * S, s1 * S
+        x = qkv[r0:r1].double().view(n, S, 3, heads, 64)
+        q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))          # n, heads, S, 64
+        sc = q @ k.transpose(-1, -2) / 8.0
+        if amd is not None:
+            sc = sc.masked_fill(amd[s0:s1].view(n, 1, 1, S) == 0, float("-inf"))
+        if late_max:
+            blk = 128 if S > 256 else 64
+            assert bool((sc.argmax(-1) >= blk * ((S - 1) // blk)).all()), "late_max: a row peaks before the last block"
+        lse_r = torch.logsumexp(sc, -1)
+        p = torch.exp(sc - lse_r[..., None])
+        mult = None if keep is None else keep[s0:s1].double() / (1.0 - round(dropout * 65536) / 65536.0)
+        pm = p if mult is None else p * mult
+        o = pm @ v
+        dO = dctx[r0:r1].double().view(n, S, heads, 64).transpose(1, 2)
+        dp = dO @ v.transpose(-1, -2)
+        if mult is not None:
+            dp = dp * mult
+        ds = p * (dp - (p * dp).sum(-1, keepdim=True)) / 8.0
+        got = dqkv[r0:r1].view(n, S, 3, heads, 64)
+        c_got = ctx[r0:r1].view(n, S, heads, 64).transpose(1, 2).double()
+        dD = (dO.abs() * (c_got - o).abs()).sum(-1, keepdim=True) if S > 256 else 0.0
+        A = p * (2 ** -12 * (dp.abs() + (p * dp.abs()).sum(-1, keepdim=True)) + dD) / 8.0
+        _per_problem("ctx", c_got, o, 2 ** -7, 1e-4, res)
+        _per_problem("lse", lse[s0:s1].double()[..., None], lse_r[..., None], 0.0, 1e-4, res)
+        _per_problem("dq", got[:, :, 0].transpose(1, 2).double(), ds @ k, 2 ** -6, 1e-5, res, A @ k.abs())
+        _per_problem("dk", got[:, :, 1].transpose(1, 2).double(), ds.transpose(-1, -2) @ q, 2 ** -6, 1e-5, res,
+                     A.transpose(-1, -2) @ q.abs())
+        _per_problem("dv", got[:, :, 2].transpose(1, 2).double(), pm.transpose(-1, -2) @ dO, 2 ** -6, 1e-5, res)
+        del x, q, k, v, sc, p, pm, o, dO, dp, ds, got, c_got, A, mult
+    want = 1 + dqkv.double().sum(0)
+    res["dbias_err"], res["dbias_scale"] = float((dbias.double() - want).abs().max()), float(want.abs().max())
+    res["dbias_ratio"] = res["dbias_err"] / (1e-5 * res["dbias_scale"])
+    bad = [f"{k[:-6]}: err {res[k[:-6] + '_err']:.3e} at max|ref| {res[k[:-6] + '_scale']:.3e} ({v:.2f} x gate)"
+           for k, v in res.items() if k.endswith("_ratio") and v > 1.0]
+    assert not bad, "; ".join(bad)
     return res
 
 

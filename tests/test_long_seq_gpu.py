@@ -1,9 +1,9 @@
 """Sequences of 256 < S <= 512 tokens on the GPU: the key-blocked attention kernels (csrc/attention_long.cu), the
 16-keys-per-lane pruned last layer (csrc/cls_last.cu) and the assembled encoder.
 
-  * kernel parity against the CPU oracle (tests/gpu_checks.check_attention: ctx 2^-7, lse 1e-4, dqkv 2^-6 of max|ref|
-    + atol, fused QKV bias gradient), with and without a padding mask, many problems, and attention-probability dropout
-    with the mask replayed from dprb_dropout_mask;
+  * kernel parity against float64 (tests/gpu_checks.check_attention: ctx 2^-7, lse 1e-4, dQ / dK / dV 2^-6 of each
+    (sequence, head) problem's max|ref| + atol, fused QKV bias gradient), with and without a padding mask, many
+    problems, and attention-probability dropout with the mask replayed from dprb_dropout_mask;
   * the two-kernel backward is deterministic; S = 513 is rejected before any launch;
   * BERT-base at S = 512 (sequence 0 uses position 511) against the reference-generated golden, with the gates of
     tests/test_realdims_gpu.py;
