@@ -156,6 +156,14 @@ int dprb_encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b,
                      int layer_lo, int layer_hi, dprb_stream_t stream) {
   return encoder_bwd(w, b, dpooled, layer_lo, layer_hi, S(stream));
 }
+int dprb_encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_batch* b, void* tokens,
+                            dprb_stream_t stream) {
+  return encoder_fwd_tokens(w, b, tokens, S(stream));
+}
+int dprb_maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_t* d_mask, const int32_t* q_index,
+                    int nq, int SQ, int B, int SD, int P, int pool, float* score, dprb_stream_t stream) {
+  return maxsim_fwd(q, d, q_mask, d_mask, q_index, nq, SQ, B, SD, P, pool, score, S(stream));
+}
 int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
                          int H, int L, dprb_stream_t stream) {
   return seqcls_head_fwd(pre, weight, bias, logits, score, N, H, L, S(stream));

@@ -109,5 +109,9 @@ long long encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S
 int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, cudaStream_t stream);
 int encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, const float* dpooled, int layer_lo,
                 int layer_hi, cudaStream_t stream);
+int encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_batch* b, void* tokens, cudaStream_t stream);
+
+int maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_t* d_mask, const int32_t* q_index,
+               int nq, int SQ, int B, int SD, int P, int pool, float* score, cudaStream_t stream);
 
 }  // namespace dprb

@@ -125,7 +125,13 @@ long long encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S
   return ws.bytes;
 }
 
-int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, cudaStream_t stream) {
+namespace {
+
+// The layer stack of both forward entry points.  pooled != nullptr: CLS output (fp32 [nseq, H]), last layer CLS-pruned
+// unless DPRB_NO_CLS_PRUNE is set.  tokens != nullptr: every token of the last layer, bf16 [nseq*S, H], written by the
+// final LayerNorm straight into the caller's buffer; the last layer is never pruned.
+int forward_layers(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, bf16* tokens,
+                   cudaStream_t stream) {
   Workspace ws;
   TRY(plan(w, b->nseq, b->S, b->save_for_backward, b->workspace, &ws));
   // position ids index a table of max_pos rows (RoBERTa's pad-derived ids need max_pos >= S + pad + 1: checked by the caller)
@@ -146,7 +152,7 @@ int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, floa
   for (int l = 0; l < L; ++l) {
     const LayerW lw = layer_w(w, l);
     LayerActs& a = ws.slot[b->save_for_backward ? l : (l & 1)];
-    if (l == L - 1 && prune_last_layer()) {
+    if (l == L - 1 && tokens == nullptr && prune_last_layer()) {
       // Last layer: only token 0 of each sequence is consumed downstream (hf_model.py:39).  K and V are needed for all
       // tokens, everything after the attention scores only for the nseq CLS rows (stored in the first nseq rows of
       // this layer's activation buffers; the saved probabilities reuse the lse buffer).
@@ -168,10 +174,23 @@ int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, floa
     TRY(gemm_bf16(a.x1, lw.w1, a.hact, T, I, H, H, H, I, 0, 0, GELU_EPI, lw.b1, nullptr, 0, a.hpre, 1.f, 1, nullptr, 0.f, 0, stream));
     TRY(gemm_bf16(a.hact, lw.w2, a.z2, T, H, I, I, I, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.b2, ws.rB, H, nullptr, 1.f, 1, nullptr, dp, site_seed(b, l, DROP_SITE_FFN_OUT), stream));
     const bool last = (l == L - 1);
-    TRY(ln_fwd(a.z2, lw.ln2g, lw.ln2b, a.out, a.stats2, last ? pooled : nullptr, b->S, T, H, w->ln_eps, RS_F16, last ? nullptr : ws.rA, stream));
-    x = a.out;
+    bf16* y = (last && tokens != nullptr) ? tokens : a.out;
+    TRY(ln_fwd(a.z2, lw.ln2g, lw.ln2b, y, a.stats2, last ? pooled : nullptr, b->S, T, H, w->ln_eps, RS_F16, last ? nullptr : ws.rA, stream));
+    x = y;
   }
   return 0;
+}
+
+}  // namespace
+
+int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, cudaStream_t stream) {
+  return forward_layers(w, b, pooled, nullptr, stream);
+}
+
+int encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_batch* b, void* tokens, cudaStream_t stream) {
+  DPRB_REQUIRE(b->save_for_backward == 0, "encoder_fwd_tokens: forward only (save_for_backward must be 0)");
+  DPRB_REQUIRE(tokens != nullptr || (long long)b->nseq * b->S == 0, "encoder_fwd_tokens: tokens output is NULL");
+  return forward_layers(w, b, nullptr, reinterpret_cast<bf16*>(tokens), stream);
 }
 
 int encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, const float* dpooled, int layer_lo,

@@ -3,6 +3,8 @@
 PyTorch is plumbing here: device memory, streams, autograd bookkeeping.  Every function launches
 hand-written sm_90a kernels from libdprb.so; nothing falls back to torch math.
 """
+import ctypes
+
 import torch
 
 from . import _lib
@@ -335,3 +337,52 @@ def topk_merge(scores, index, k):
     check(lib.dprb_topk_merge(_ptr(scores), _ptr(index), Q, total, int(k), _ptr(out_s), _ptr(out_i), _ptr(ws),
                               ws.numel(), _stream()), "dprb_topk_merge")
     return out_s, out_i
+
+
+def encoder_fwd_tokens(w, b, out):
+    """Token-level encoder forward: every token of the last layer, bf16 [nseq*S, H] written into `out` (contiguous
+    CUDA).  w / b: the dprb_encoder_weights / dprb_encoder_batch structs (b.save_for_backward must be 0)."""
+    check(_lib.load().dprb_encoder_fwd_tokens(ctypes.byref(w), ctypes.byref(b), _ptr(out), _stream()),
+          "dprb_encoder_fwd_tokens")
+    return out
+
+
+MAXSIM_POOLS = {"sum": 0, "max": 1}   # include/dprb.h DPRB_MAXSIM_SUM / DPRB_MAXSIM_MAX
+MAXSIM_MAX_S, MAXSIM_MAX_P = 512, 1024
+
+
+def maxsim_check(SQ, SD, P):
+    """ValueError for the shapes dprb_maxsim_fwd refuses (token 0 of each side is skipped)."""
+    if P % 8 or not 8 <= P <= MAXSIM_MAX_P:
+        raise ValueError(f"MaxSim needs the token dimension to be a multiple of 8 and at most {MAXSIM_MAX_P} (got {P})")
+    for name, S in (("query", SQ), ("passage", SD)):
+        if not 2 <= S <= MAXSIM_MAX_S:
+            raise ValueError(f"MaxSim needs {name} sequences of 2 .. {MAXSIM_MAX_S} tokens (got {S})")
+
+
+def maxsim(q, d, q_mask, d_mask, q_index, pool="sum"):
+    """ColBERT MaxSim scores of pairs: q bf16 [nq, SQ, P] (projected query tokens), d bf16 [B, SD, P] (passage tokens),
+    int masks [nq, SQ] / [B, SD] (None: every token real), q_index [B] (the query row of each pair; a CPU tensor is
+    range-checked without a device sync) -> score fp32 [B] = sum (or max) over query tokens 1.. of the max over passage
+    tokens 1.. of q . d, masked tokens counting as zero vectors (include/dprb.h dprb_maxsim_fwd)."""
+    if pool not in MAXSIM_POOLS:
+        raise ValueError(f"MaxSim pool must be one of {sorted(MAXSIM_POOLS)} (got {pool!r})")
+    if q.dim() != 3 or d.dim() != 3 or q.shape[2] != d.shape[2]:
+        raise ValueError(f"MaxSim needs q [nq, SQ, P] and d [B, SD, P] (got {tuple(q.shape)} and {tuple(d.shape)})")
+    nq, SQ, P = q.shape
+    B, SD, _ = d.shape
+    maxsim_check(SQ, SD, P)
+    q_index = torch.as_tensor(q_index)
+    if q_index.shape != (B,):
+        raise ValueError(f"MaxSim needs one query index per pair ({B}), got shape {tuple(q_index.shape)}")
+    if B and (int(q_index.min()) < 0 or int(q_index.max()) >= nq):
+        raise ValueError(f"MaxSim query indices must lie in [0, {nq})")
+    assert q.dtype == d.dtype == torch.bfloat16 and q.is_contiguous() and d.is_contiguous()
+    dev = d.device
+    idx = q_index.to(dev, torch.int32).contiguous()
+    qm = None if q_mask is None else q_mask.to(dev, torch.int32).contiguous()
+    dm = None if d_mask is None else d_mask.to(dev, torch.int32).contiguous()
+    score = torch.empty(B, dtype=torch.float32, device=dev)
+    check(_lib.load().dprb_maxsim_fwd(_ptr(q), _ptr(d), _ptr(qm), _ptr(dm), _ptr(idx), nq, SQ, B, SD, P,
+                                      MAXSIM_POOLS[pool], _ptr(score), _stream()), "dprb_maxsim_fwd")
+    return score

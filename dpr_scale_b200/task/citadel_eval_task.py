@@ -1,0 +1,90 @@
+"""RerankMultiVecRetrieverTask — drop-in for ``dpr_scale.task.citadel_eval_task.RerankMultiVecRetrieverTask``
+(/root/reference/dpr_scale/task/citadel_eval_task.py:215-313) with ColBERT encoders: scores every (query, passage) row
+of a TREC run by late interaction and writes ``scores_{rank:04}.pkl`` (fp32 CPU tensor ``[n]``), ``qids_{rank:04}.pkl``
+and ``ctx_ids_{rank:04}.pkl`` (lists), pickle protocol 4, in the row order of the rank's shard.
+``python -m dpr_scale_b200.rerank`` merges them into a run file.
+
+Accepts the keywords of the reference's ``MultiVecRetrieverTask`` (dpr_scale/task/citadel_task.py:8-24) on top of
+DenseRetrieverTask's; only ``query_pool`` ("sum" or "max") changes what an eval step computes - the others belong to
+training or to CITADEL / COIL routing, which ColBERT does not use.  ``setup`` builds the two encoders and strictly loads
+``checkpoint_path`` (a Lightning checkpoint with a ``state_dict``).
+
+An eval step never materialises ``expert_repr``: each distinct query of the batch is encoded once (rows are encoded
+independently at the batch's padded width, so this equals encoding every row), the passages are encoded, both are
+projected by the library's GEMM, and ``dprb_maxsim_fwd`` scores the pairs from the unmasked tokens and the masks.
+"""
+import os
+import pickle
+
+import torch
+import torch.distributed as dist
+
+from .. import ops
+from .dpr_task import DenseRetrieverTask
+
+
+class RerankMultiVecRetrieverTask(DenseRetrieverTask):
+    def __init__(self, checkpoint_path, output_dir, add_cls: bool = False, query_topk: int = 1, context_topk: int = 1,
+                 query_expert_load_loss_coef: float = 0, context_expert_load_loss_coef: float = 0,
+                 query_router_marg_load_loss_coef: float = 0, context_router_marg_load_loss_coef: float = 0,
+                 cross_batch: bool = True, in_batch: bool = True, query_pool: str = "sum", anneal_factor: float = 0.0,
+                 teacher_coef: float = 0.0, tau: float = 1.0, **kwargs):
+        super().__init__(**kwargs)
+        self.query_pool = query_pool
+        self.checkpoint_path = checkpoint_path
+        self.output_dir = output_dir
+        self.dedupe_queries = True      # False: encode every row's query (the same scores, bit for bit)
+        os.makedirs(output_dir, exist_ok=True)
+
+    def setup(self, stage: str):
+        if self.setup_done:
+            return
+        super().setup("train")
+        print(f"Loading checkpoint from {self.checkpoint_path}")
+        ckpt = torch.load(self.checkpoint_path, map_location="cpu", weights_only=False)
+        self.load_state_dict(ckpt["state_dict"])
+
+    def _scores(self, batch):
+        if self.query_pool not in ops.MAXSIM_POOLS:
+            raise NotImplementedError("Invalid query pooling! Available: [max, sum]")
+        q_tok, c_tok = batch["query_ids"], batch["contexts_ids"]
+        n = len(batch["qid"])
+        index = list(range(n))
+        if self.dedupe_queries:
+            first, rows = {}, []
+            for i, q in enumerate(batch["qid"]):
+                if q not in first:
+                    first[q] = len(rows)
+                    rows.append(i)
+                index[i] = first[q]
+            if len(rows) < n:
+                q_tok = {k: v[torch.tensor(rows, device=v.device)] for k, v in q_tok.items()}
+        with torch.no_grad():
+            q, q_mask = self.query_encoder.token_reps(q_tok)
+            d, d_mask = self.context_encoder.token_reps(c_tok)
+            return ops.maxsim(q, d, q_mask, d_mask, torch.tensor(index, dtype=torch.int32), self.query_pool)
+
+    def _eval_step(self, batch, batch_idx):
+        return [batch["qid"], batch["ctx_id"], self._scores(batch).cpu()]
+
+    def test_step(self, batch, batch_idx):
+        return self._eval_step(batch, batch_idx)
+
+    def _out(self, what):
+        return os.path.join(self.output_dir, f"{what}_{self.global_rank:04}.pkl")
+
+    def test_epoch_end(self, test_outputs):
+        qids, ctx_ids, scores = [], [], []
+        for b_qids, b_ctx_ids, b_scores in test_outputs:
+            qids.extend(b_qids)
+            ctx_ids.extend(b_ctx_ids)
+            scores.append(b_scores)
+        scores = torch.cat(scores, dim=0) if scores else torch.zeros(0, dtype=torch.float32)
+        out_file = self._out("scores")
+        print(f"\nWriting scores to {out_file}")
+        for what, obj in (("scores", scores), ("qids", qids), ("ctx_ids", ctx_ids)):
+            with open(self._out(what), "wb") as f:
+                pickle.dump(obj, f, protocol=4)
+        if dist.is_available() and dist.is_initialized():
+            dist.barrier()                            # rank 0 merges only once every shard is on disk
+        return out_file

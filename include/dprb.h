@@ -271,6 +271,30 @@ int dprb_encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b,
 int dprb_encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, const float* dpooled,
                      int layer_lo, int layer_hi, dprb_stream_t stream);
 
+/* Token-level forward (ColBERT / late-interaction encoders: dpr_scale/models/citadel_models/colbert_model.py:39-44
+ * reads hidden_states[-1]).  Writes the final LayerNorm output of EVERY token, bf16 [nseq*S, hidden] row-major, straight
+ * into `tokens`; the last layer is never CLS-pruned, whatever DPRB_NO_CLS_PRUNE says.  Forward only: returns 1 unless
+ * b->save_for_backward == 0.  Workspace: dprb_encoder_workspace_bytes(w, nseq, S, 0).  Row s*S of `tokens` equals
+ * bf16(pooled[s]) of dprb_encoder_fwd run with DPRB_NO_CLS_PRUNE=1 on the same batch, bit for bit. */
+int dprb_encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_batch* b, void* tokens,
+                            dprb_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Late-interaction (ColBERT MaxSim) scores of reranking pairs, forward only.  Replaces expert_sim_score of
+ * dpr_scale/task/citadel_eval_task.py:236-265 (no expert ids): for pair b with query qi = q_index[b],
+ *   s[i][j] = q[qi][i] . d[b][j]            over tokens i = 1 .. SQ-1, j = 1 .. SD-1 (token 0 is skipped)
+ *   score[b] = sum_i max_j s[i][j]          (pool DPRB_MAXSIM_SUM)   or   max_i max_j s[i][j]   (DPRB_MAXSIM_MAX)
+ * with the reference's zero-vector padding: a masked passage token (d_mask 0) scores exactly 0 and takes part in the
+ * max; a masked query token contributes exactly 0 (sum) or offers 0 (max).  Masks may be NULL (every token real).
+ *   q bf16 [nq, SQ, P], d bf16 [B, SD, P] row-major, 16-byte aligned; q_mask int32 [nq, SQ], d_mask int32 [B, SD];
+ *   q_index int32 [B] (device), each in [0, nq): the caller checks this (an index out of range gives a NaN score);
+ *   score fp32 [B].  bf16 products, fp32 accumulation; scores are bitwise repeatable (fixed reduction order).
+ * Requires P % 8 == 0, P <= 1024, 2 <= SQ, SD <= 512 (checked before any launch, return code 1). */
+#define DPRB_MAXSIM_SUM 0
+#define DPRB_MAXSIM_MAX 1
+int dprb_maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_t* d_mask, const int32_t* q_index,
+                    int nq, int SQ, int B, int SD, int P, int pool, float* score, dprb_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Cross-encoder sequence-classification head (reranking: dpr_scale/models/citadel_models/cross_encoder.py:21-26,
  * AutoModelForSequenceClassification under no_grad).  The caller runs the head's dense layer first, on the CLS rows
