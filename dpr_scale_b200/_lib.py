@@ -88,6 +88,8 @@ SIGNATURES = {
     "dprb_encoder_bwd": (c_int, [POINTER(EncoderWeights), POINTER(EncoderBatch), _P, c_int, c_int, _P]),
     "dprb_encoder_fwd_tokens": (c_int, [POINTER(EncoderWeights), POINTER(EncoderBatch), _P, _P]),
     "dprb_maxsim_fwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P]),
+    "dprb_maxsim_expert_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int,
+                                       c_int, c_int, c_int, _P, _P]),
     "dprb_seqcls_head_fwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
     "dprb_search_workspace_bytes": (c_int64, [c_int64, c_int]),
     "dprb_search_topk": (c_int, [_P, _P, c_int, c_int64, c_int64, c_int, c_int, c_int64, _P, _P, _P, c_int64, _P]),

@@ -164,6 +164,13 @@ int dprb_maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const i
                     int nq, int SQ, int B, int SD, int P, int pool, float* score, dprb_stream_t stream) {
   return maxsim_fwd(q, d, q_mask, d_mask, q_index, nq, SQ, B, SD, P, pool, score, S(stream));
 }
+int dprb_maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const float* q_w, const int32_t* d_ids,
+                           const float* d_w, const void* q_cls, const void* d_cls, const int32_t* q_index, int nq,
+                           int SQ, int B, int SD, int P, int KQ, int KD, int Pc, int pool, float* score,
+                           dprb_stream_t stream) {
+  return maxsim_expert_fwd(q, d, q_ids, q_w, d_ids, d_w, q_cls, d_cls, q_index, nq, SQ, B, SD, P, KQ, KD, Pc, pool,
+                           score, S(stream));
+}
 int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
                          int H, int L, dprb_stream_t stream) {
   return seqcls_head_fwd(pre, weight, bias, logits, score, N, H, L, S(stream));

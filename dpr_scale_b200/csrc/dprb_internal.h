@@ -113,5 +113,8 @@ int encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_batch* 
 
 int maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_t* d_mask, const int32_t* q_index,
                int nq, int SQ, int B, int SD, int P, int pool, float* score, cudaStream_t stream);
+int maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const float* q_w, const int32_t* d_ids,
+                      const float* d_w, const void* q_cls, const void* d_cls, const int32_t* q_index, int nq, int SQ,
+                      int B, int SD, int P, int KQ, int KD, int Pc, int pool, float* score, cudaStream_t stream);
 
 }  // namespace dprb

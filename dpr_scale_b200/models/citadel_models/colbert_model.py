@@ -28,6 +28,39 @@ from ..hf_model import HFEncoder, ParamLayout, _normalise_config
 _KINDS = ("bert", "roberta", "xlm-roberta")
 
 
+def encode_tokens(body: HFEncoder, tokens):
+    """(hidden bf16 [N*S, H], mask int32 [N, S], N, S): every token of the last layer of ``body``
+    (dprb_encoder_fwd_tokens, eval mode)."""
+    ids, tt, pos, am, N, S = body._prep_tokens(tokens)
+    body._ensure_device_state(False)
+    ws = body._workspace(N, S, False)
+    base = (ws.data_ptr() + 255) & ~255
+    b = EncoderBatch()
+    b.nseq, b.S = N, S
+    b.ids, b.type_ids, b.pos_ids = ids.data_ptr(), tt.data_ptr(), pos.data_ptr()
+    b.attn_mask = am.data_ptr() if am is not None else None
+    b.workspace, b.workspace_bytes = base, ws.numel() - (base - ws.data_ptr())
+    b.save_for_backward, b.dropout_p, b.dropout_seed = 0, 0.0, 0      # eval: dropout is the identity
+    H = body.config["hidden_size"]
+    hidden = torch.empty(N * S, H, dtype=torch.bfloat16, device=ids.device)
+    ops.encoder_fwd_tokens(body._weights_struct(False), b, hidden)
+    body.launches += 1 + 7 * body.config["num_hidden_layers"]
+    if am is None:
+        am = torch.ones(N, S, dtype=torch.int32, device=ids.device)
+    return hidden, am, N, S
+
+
+def linear_bf16(lin: nn.Linear, x):
+    """bf16 [T, out] = x @ lin.weight^T + lin.bias: x bf16 [T, in] contiguous, on the library's GEMM (bias epilogue)."""
+    T, K = x.shape
+    N = lin.out_features
+    w16 = torch.empty(N, K, dtype=torch.bfloat16, device=x.device)
+    ops.cast_f32_bf16(lin.weight.detach().contiguous(), w16)
+    y = torch.empty(T, N, dtype=torch.bfloat16, device=x.device)
+    ops.gemm(x, w16, y, T, N, K, K, K, N, False, False, ops.EPI_BIAS, lin.bias.detach().contiguous())
+    return y
+
+
 class ColBERTEncoder(nn.Module):
     def __init__(self, model_path: str = "roberta-base", dropout: float = 0.1, projection_dim: Optional[int] = None,
                  _config=None, _seed: int = 0):
@@ -84,43 +117,27 @@ class ColBERTEncoder(nn.Module):
     # ------------------------------------------------------------------ forward
     def _check_call(self, tokens):
         if torch.is_grad_enabled():
-            raise ValueError("ColBERTEncoder runs forward only (training is not implemented): call it under "
+            raise ValueError(f"{type(self).__name__} runs forward only (training is not implemented): call it under "
                              "torch.no_grad()")
         S = tokens["input_ids"].shape[-1]
         if not 2 <= S <= ops.MAXSIM_MAX_S:
-            raise ValueError(f"ColBERTEncoder needs 2 .. {ops.MAXSIM_MAX_S} tokens per sequence (got {S}): token 0 "
-                             "is dropped")
+            raise ValueError(f"{type(self).__name__} needs 2 .. {ops.MAXSIM_MAX_S} tokens per sequence (got {S}): "
+                             "token 0 is dropped")
 
     def token_reps(self, tokens):
         """(reps bf16 [N, S, P], mask int32 [N, S]): projected last-layer tokens, token 0 included and padded tokens not
         zeroed (their mask is 0)."""
-        self._check_call(tokens)
-        body = self._body
-        ids, tt, pos, am, N, S = body._prep_tokens(tokens)
-        body._ensure_device_state(False)
-        ws = body._workspace(N, S, False)
-        base = (ws.data_ptr() + 255) & ~255
-        b = EncoderBatch()
-        b.nseq, b.S = N, S
-        b.ids, b.type_ids, b.pos_ids = ids.data_ptr(), tt.data_ptr(), pos.data_ptr()
-        b.attn_mask = am.data_ptr() if am is not None else None
-        b.workspace, b.workspace_bytes = base, ws.numel() - (base - ws.data_ptr())
-        b.save_for_backward, b.dropout_p, b.dropout_seed = 0, 0.0, 0      # eval: dropout is the identity
+        hidden, am, N, S = self._hidden(tokens)
         H = self.config["hidden_size"]
-        hidden = torch.empty(N * S, H, dtype=torch.bfloat16, device=ids.device)
-        ops.encoder_fwd_tokens(body._weights_struct(False), b, hidden)
-        body.launches += 1 + 7 * self.config["num_hidden_layers"]
-        if am is None:
-            am = torch.ones(N, S, dtype=torch.int32, device=ids.device)
         if isinstance(self.project, nn.Identity):
             return hidden.view(N, S, H), am
-        lin = self.project[0]
-        P = lin.out_features
-        w16 = torch.empty(P, H, dtype=torch.bfloat16, device=ids.device)
-        ops.cast_f32_bf16(lin.weight.detach().contiguous(), w16)
-        reps = torch.empty(N * S, P, dtype=torch.bfloat16, device=ids.device)
-        ops.gemm(hidden, w16, reps, N * S, P, H, H, H, P, False, False, ops.EPI_BIAS, lin.bias.detach().contiguous())
-        return reps.view(N, S, P), am
+        reps = linear_bf16(self.project[0], hidden)
+        return reps.view(N, S, -1), am
+
+    def _hidden(self, tokens):
+        """(hidden bf16 [N*S, H], mask int32 [N, S], N, S): the last layer of every token."""
+        self._check_call(tokens)
+        return encode_tokens(self._body, tokens)
 
     def forward(self, tokens, **kwargs):
         reps, am = self.token_reps(tokens)

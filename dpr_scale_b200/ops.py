@@ -386,3 +386,64 @@ def maxsim(q, d, q_mask, d_mask, q_index, pool="sum"):
     check(_lib.load().dprb_maxsim_fwd(_ptr(q), _ptr(d), _ptr(qm), _ptr(dm), _ptr(idx), nq, SQ, B, SD, P,
                                       MAXSIM_POOLS[pool], _ptr(score), _stream()), "dprb_maxsim_fwd")
     return score
+
+
+MAXSIM_MAX_EXPERTS = 8   # include/dprb.h dprb_maxsim_expert_fwd: 1 <= KQ, KD <= 8
+
+
+def maxsim_expert_check(SQ, SD, P, KQ, KD, Pc=None):
+    """ValueError for the shapes dprb_maxsim_expert_fwd refuses (Pc: the CLS width, None without a CLS term)."""
+    maxsim_check(SQ, SD, P)
+    for name, K in (("query", KQ), ("passage", KD)):
+        if not 1 <= K <= MAXSIM_MAX_EXPERTS:
+            raise ValueError(f"expert MaxSim needs 1 .. {MAXSIM_MAX_EXPERTS} experts per {name} token (got {K})")
+    if Pc is not None and (Pc % 8 or not 8 <= Pc <= MAXSIM_MAX_P):
+        raise ValueError(f"expert MaxSim needs the CLS dimension to be a multiple of 8 and at most {MAXSIM_MAX_P} "
+                         f"(got {Pc})")
+
+
+def maxsim_expert(q, d, q_ids, q_w, d_ids, d_w, q_index, pool="sum", q_cls=None, d_cls=None):
+    """COIL / CITADEL scores of pairs (include/dprb.h dprb_maxsim_expert_fwd): q bf16 [nq, SQ, P], d bf16 [B, SD, P]
+    (unmasked tokens, token 0 included), expert ids [nq, SQ, KQ] / [B, SD, KD] (int) and weights (fp32, 0 on masked
+    tokens) of the same shape, q_index [B] (a CPU tensor is range-checked without a device sync), optional CLS vectors
+    bf16 [nq, Pc] / [B, Pc] -> score fp32 [B] = sum (or max) over query rows (i, a) of the max over passage columns
+    (j, b) of q_i . d_j * wq[i, a] * wd[j, b] where the ids agree and 0 where they differ, plus q_cls . d_cls."""
+    if pool not in MAXSIM_POOLS:
+        raise ValueError(f"MaxSim pool must be one of {sorted(MAXSIM_POOLS)} (got {pool!r})")
+    if q.dim() != 3 or d.dim() != 3 or q.shape[2] != d.shape[2]:
+        raise ValueError(f"MaxSim needs q [nq, SQ, P] and d [B, SD, P] (got {tuple(q.shape)} and {tuple(d.shape)})")
+    nq, SQ, P = q.shape
+    B, SD, _ = d.shape
+    if q_ids.dim() != 3 or q_ids.shape[:2] != (nq, SQ) or q_w.shape != q_ids.shape:
+        raise ValueError(f"expert MaxSim needs query ids and weights [{nq}, {SQ}, KQ] (got {tuple(q_ids.shape)} and "
+                         f"{tuple(q_w.shape)})")
+    if d_ids.dim() != 3 or d_ids.shape[:2] != (B, SD) or d_w.shape != d_ids.shape:
+        raise ValueError(f"expert MaxSim needs passage ids and weights [{B}, {SD}, KD] (got {tuple(d_ids.shape)} and "
+                         f"{tuple(d_w.shape)})")
+    if (q_cls is None) != (d_cls is None):
+        raise ValueError("expert MaxSim needs both CLS operands or neither")
+    Pc = None
+    if q_cls is not None:
+        Pc = q_cls.shape[-1]
+        if q_cls.shape != (nq, Pc) or d_cls.shape != (B, Pc):
+            raise ValueError(f"expert MaxSim needs CLS vectors [{nq}, Pc] and [{B}, Pc] (got {tuple(q_cls.shape)} and "
+                             f"{tuple(d_cls.shape)})")
+    maxsim_expert_check(SQ, SD, P, q_ids.shape[2], d_ids.shape[2], Pc)
+    q_index = torch.as_tensor(q_index)
+    if q_index.shape != (B,):
+        raise ValueError(f"MaxSim needs one query index per pair ({B}), got shape {tuple(q_index.shape)}")
+    if B and (int(q_index.min()) < 0 or int(q_index.max()) >= nq):
+        raise ValueError(f"MaxSim query indices must lie in [0, {nq})")
+    assert q.dtype == d.dtype == torch.bfloat16 and q.is_contiguous() and d.is_contiguous()
+    if q_cls is not None:
+        assert q_cls.dtype == d_cls.dtype == torch.bfloat16 and q_cls.is_contiguous() and d_cls.is_contiguous()
+    dev = d.device
+    idx = q_index.to(dev, torch.int32).contiguous()
+    qi, qw = q_ids.to(dev, torch.int32).contiguous(), q_w.to(dev, torch.float32).contiguous()
+    di, dw = d_ids.to(dev, torch.int32).contiguous(), d_w.to(dev, torch.float32).contiguous()
+    score = torch.empty(B, dtype=torch.float32, device=dev)
+    check(_lib.load().dprb_maxsim_expert_fwd(_ptr(q), _ptr(d), _ptr(qi), _ptr(qw), _ptr(di), _ptr(dw), _ptr(q_cls),
+                                             _ptr(d_cls), _ptr(idx), nq, SQ, B, SD, P, qi.shape[2], di.shape[2],
+                                             0 if Pc is None else Pc, MAXSIM_POOLS[pool], _ptr(score), _stream()),
+          "dprb_maxsim_expert_fwd")
+    return score

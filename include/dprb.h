@@ -295,6 +295,25 @@ int dprb_encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_ba
 int dprb_maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_t* d_mask, const int32_t* q_index,
                     int nq, int SQ, int B, int SD, int P, int pool, float* score, dprb_stream_t stream);
 
+/* Expert-matched late interaction (COIL / CITADEL rerankers): the expert-id branch of expert_sim_score,
+ * dpr_scale/task/citadel_eval_task.py:240-258, plus the CLS term of _eval_step (:282-283).  Query token i (1 .. SQ-1) has
+ * KQ (expert id, weight) pairs, passage token j (1 .. SD-1) has KD; with s[i][j] = q[qi][i] . d[b][j],
+ *   e[(i,a)][(j,b)] = s[i][j] * (wq[i][a] * wd[j][b])   where q_ids[i][a] == d_ids[j][b], exactly 0 where they differ
+ *   score[b] = sum over rows (i,a) of max over columns (j,b) of e   (DPRB_MAXSIM_SUM; max over rows for DPRB_MAXSIM_MAX)
+ *            + sum_k q_cls[qi][k] * d_cls[b][k]                      (fp32; only when q_cls / d_cls are given)
+ * The zeros of unmatched entries take part in the max, as in the reference.  Masks enter through the weights: give a
+ * masked token weight 0 on its side (its ids are then irrelevant), which reproduces the reference's zero-vector padding.
+ *   q / d / q_index / score as in dprb_maxsim_fwd (q and d are the unmasked tokens);
+ *   q_ids int32 / q_w fp32 [nq, SQ, KQ], d_ids int32 / d_w fp32 [B, SD, KD] (entries of token 0 are not read);
+ *   q_cls bf16 [nq, Pc], d_cls bf16 [B, Pc], 16-byte aligned, or both NULL (Pc is then ignored).
+ * With KQ = KD = 1, equal ids and the 0/1 masks as weights, the scores equal dprb_maxsim_fwd's bit for bit.  Bitwise
+ * repeatable.  Requires P % 8 == 0, P <= 1024, 2 <= SQ, SD <= 512, 1 <= KQ, KD <= 8 and, with CLS operands,
+ * Pc % 8 == 0, Pc <= 1024 (checked before any launch, return code 1). */
+int dprb_maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const float* q_w, const int32_t* d_ids,
+                           const float* d_w, const void* q_cls, const void* d_cls, const int32_t* q_index, int nq,
+                           int SQ, int B, int SD, int P, int KQ, int KD, int Pc, int pool, float* score,
+                           dprb_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Cross-encoder sequence-classification head (reranking: dpr_scale/models/citadel_models/cross_encoder.py:21-26,
  * AutoModelForSequenceClassification under no_grad).  The caller runs the head's dense layer first, on the CLS rows
