@@ -171,6 +171,10 @@ int dprb_maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, c
   return maxsim_expert_fwd(q, d, q_ids, q_w, d_ids, d_w, q_cls, d_cls, q_index, nq, SQ, B, SD, P, KQ, KD, Pc, pool,
                            score, S(stream));
 }
+int dprb_splade_pool_fwd(const void* x, int64_t ldx, const void* W, int64_t ldw, const float* bias, const int32_t* off,
+                         int64_t T, int N, int V, int K, float* out, int64_t ldo, dprb_stream_t stream) {
+  return splade_pool_fwd(x, ldx, W, ldw, bias, off, T, N, V, K, out, ldo, S(stream));
+}
 int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
                          int H, int L, dprb_stream_t stream) {
   return seqcls_head_fwd(pre, weight, bias, logits, score, N, H, L, S(stream));

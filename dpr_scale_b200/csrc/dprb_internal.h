@@ -117,4 +117,7 @@ int maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const 
                       const float* d_w, const void* q_cls, const void* d_cls, const int32_t* q_index, int nq, int SQ,
                       int B, int SD, int P, int KQ, int KD, int Pc, int pool, float* score, cudaStream_t stream);
 
+int splade_pool_fwd(const void* x, long long ldx, const void* W, long long ldw, const float* bias, const int32_t* off,
+                    long long T, int N, int V, int K, float* out, long long ldo, cudaStream_t stream);
+
 }  // namespace dprb

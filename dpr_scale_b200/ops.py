@@ -447,3 +447,51 @@ def maxsim_expert(q, d, q_ids, q_w, d_ids, d_w, q_index, pool="sum", q_cls=None,
                                              0 if Pc is None else Pc, MAXSIM_POOLS[pool], _ptr(score), _stream()),
           "dprb_maxsim_expert_fwd")
     return score
+
+
+SPLADE_MAX_K = 1024   # include/dprb.h dprb_splade_pool_fwd: K % 8 == 0, 8 <= K <= 1024
+
+
+def splade_pool_check(N, V, K, ldx=None, ldw=None, ldo=None, T=0):
+    """ValueError for the shapes dprb_splade_pool_fwd refuses (ldx / ldw default to K, ldo to V)."""
+    ldx, ldw, ldo = K if ldx is None else ldx, K if ldw is None else ldw, V if ldo is None else ldo
+    if K % 8 or not 8 <= K <= SPLADE_MAX_K:
+        raise ValueError(f"SPLADE pool needs the hidden width K to be a multiple of 8 in 8 .. {SPLADE_MAX_K} (got {K})")
+    for name, ld in (("ldx", ldx), ("ldw", ldw)):
+        if ld % 8 or ld < K:
+            raise ValueError(f"SPLADE pool needs {name} to be a multiple of 8 and at least K={K} (got {ld})")
+    if V < 1 or N < 1:
+        raise ValueError(f"SPLADE pool needs V >= 1 and N >= 1 (got V={V}, N={N})")
+    if ldo < V:
+        raise ValueError(f"SPLADE pool needs ldo >= V={V} (got {ldo})")
+    if not 0 <= T < 0x7FFFFF00:
+        raise ValueError(f"SPLADE pool needs 0 <= T < 2^31 rows (got {T})")
+
+
+def splade_pool(x, W, off, K, bias=None, out=None):
+    """SPLADE max-pool of compacted tokens (include/dprb.h dprb_splade_pool_fwd): x fp16 [T, ldx] (the tokens' head
+    transforms, rows of sequence n at off[n] .. off[n+1] - 1), W fp16 [V, ldw] (the decoder rows), off int [N + 1]
+    (non-decreasing), bias fp32 [V] or None; only the first K columns of x and W are read -> fp32 [N, V] =
+    log1p(relu(max over each sequence's rows of x . W + bias)), 0 for an empty sequence.  `out` may be a preallocated
+    fp32 [N, ldo] tensor with unit column stride (ldo >= V)."""
+    if x.dim() != 2 or W.dim() != 2 or x.dtype != torch.float16 or W.dtype != torch.float16:
+        raise ValueError("SPLADE pool needs fp16 x [T, ldx] and W [V, ldw]")
+    if x.stride(1) != 1 or W.stride(1) != 1:
+        raise ValueError("SPLADE pool needs x and W with unit column stride")
+    T, V = x.shape[0], W.shape[0]
+    off = torch.as_tensor(off)
+    N = off.numel() - 1
+    if x.shape[1] < K or W.shape[1] < K:
+        raise ValueError(f"SPLADE pool reads K={K} columns of x {tuple(x.shape)} and W {tuple(W.shape)}")
+    ldo = V if out is None else out.stride(0)
+    splade_pool_check(N, V, K, x.stride(0), W.stride(0), ldo, T)
+    dev = W.device
+    off = off.to(dev, torch.int32).contiguous()
+    if out is None:
+        out = torch.empty(N, V, dtype=torch.float32, device=dev)
+    assert out.dtype == torch.float32 and out.shape[0] >= N and out.shape[1] >= V and out.stride(1) == 1
+    b = None if bias is None else bias.to(dev, torch.float32).contiguous()
+    check(_lib.load().dprb_splade_pool_fwd(_ptr(x) if T else None, x.stride(0), _ptr(W), W.stride(0), _ptr(b),
+                                           _ptr(off), T, N, V, int(K), _ptr(out), ldo, _stream()),
+          "dprb_splade_pool_fwd")
+    return out

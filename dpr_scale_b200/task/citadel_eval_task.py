@@ -19,13 +19,12 @@ With COIL / CITADEL encoders (those with ``expert_reps``) the encoders also give
 ``dprb_maxsim_expert_fwd`` scores the pairs with the expert-matching rule and the CLS term.
 """
 import os
-import pickle
 
 import torch
-import torch.distributed as dist
 
 from .. import ops
 from .dpr_task import DenseRetrieverTask
+from .rerank_common import distinct_queries, write_rerank_pickles
 
 
 class RerankMultiVecRetrieverTask(DenseRetrieverTask):
@@ -54,19 +53,8 @@ class RerankMultiVecRetrieverTask(DenseRetrieverTask):
     def _scores(self, batch):
         if self.query_pool not in ops.MAXSIM_POOLS:
             raise NotImplementedError("Invalid query pooling! Available: [max, sum]")
-        q_tok, c_tok = batch["query_ids"], batch["contexts_ids"]
-        n = len(batch["qid"])
-        index = list(range(n))
-        if self.dedupe_queries:
-            first, rows = {}, []
-            for i, q in enumerate(batch["qid"]):
-                if q not in first:
-                    first[q] = len(rows)
-                    rows.append(i)
-                index[i] = first[q]
-            if len(rows) < n:
-                q_tok = {k: v[torch.tensor(rows, device=v.device)] for k, v in q_tok.items()}
-        index = torch.tensor(index, dtype=torch.int32)
+        c_tok = batch["contexts_ids"]
+        q_tok, index = distinct_queries(batch["qid"], batch["query_ids"], self.dedupe_queries)
         with torch.no_grad():
             if hasattr(self.query_encoder, "expert_reps"):                       # COIL / CITADEL
                 q, q_ids, q_w, q_cls = self.query_encoder.expert_reps(q_tok, topk=self.query_topk, add_cls=self.add_cls)
@@ -83,21 +71,5 @@ class RerankMultiVecRetrieverTask(DenseRetrieverTask):
     def test_step(self, batch, batch_idx):
         return self._eval_step(batch, batch_idx)
 
-    def _out(self, what):
-        return os.path.join(self.output_dir, f"{what}_{self.global_rank:04}.pkl")
-
     def test_epoch_end(self, test_outputs):
-        qids, ctx_ids, scores = [], [], []
-        for b_qids, b_ctx_ids, b_scores in test_outputs:
-            qids.extend(b_qids)
-            ctx_ids.extend(b_ctx_ids)
-            scores.append(b_scores)
-        scores = torch.cat(scores, dim=0) if scores else torch.zeros(0, dtype=torch.float32)
-        out_file = self._out("scores")
-        print(f"\nWriting scores to {out_file}")
-        for what, obj in (("scores", scores), ("qids", qids), ("ctx_ids", ctx_ids)):
-            with open(self._out(what), "wb") as f:
-                pickle.dump(obj, f, protocol=4)
-        if dist.is_available() and dist.is_initialized():
-            dist.barrier()                            # rank 0 merges only once every shard is on disk
-        return out_file
+        return write_rerank_pickles(self.output_dir, self.global_rank, test_outputs)

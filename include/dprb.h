@@ -314,6 +314,25 @@ int dprb_maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, c
                            int SQ, int B, int SD, int P, int KQ, int KD, int Pc, int pool, float* score,
                            dprb_stream_t stream);
 
+/* SPLADE vocabulary max-pool (SPLADEEncoder.forward of dpr_scale/models/citadel_models/splade_model.py after the
+ * masked-LM head's transform): the decoder GEMM with the pooling in its epilogue; the [rows, V] logits are never written.
+ *   out[n, v] = log1p( max(0, max_{r in [off[n], off[n+1])} ( x[r, :K] . W[v, :K] + bias[v] ) ) )   (0: empty range)
+ * This equals the reference's max over tokens 1.. of log(1 + relu(logit)) * attention_mask when the rows of sequence n
+ * are its valid tokens (token 0 and masked tokens dropped): every valid token contributes log(1 + relu(l)) >= 0 and
+ * every masked token exactly 0, so the masked max is log1p(relu(max over the valid tokens)), or 0 without one.
+ *   x fp16 [T, ldx], W fp16 [V, ldw], row-major, 16-byte aligned; only the first K columns are read (so the CITADEL
+ *   router's [T, H + 8] / [V, H + 8] operands serve with K = H);
+ *   bias fp32 [V], added in fp32 in the epilogue, or NULL;
+ *   off int32 [N + 1] (device), non-decreasing, off[N] <= T: the rows of sequence n are off[n] .. off[n+1] - 1; rows
+ *   before off[0] are never loaded and rows from off[N] on never enter a maximum;
+ *   out fp32 [N, ldo], ldo >= V: elements [N, V] are written (every one of them), columns >= V and rows >= N never.
+ * fp16 products, fp32 accumulation; out is bitwise repeatable and does not depend on how the sequences are grouped into
+ * calls or ordered.  Non-finite logits are out of contract.  Requires K % 8 == 0, 8 <= K <= 1024, ldx and ldw multiples
+ * of 8 and at least K, V >= 1, N >= 1, ldo >= V, 0 <= T < 2^31 (checked before any launch, return code 1).  Three
+ * launches: zero-fill, the pool, log1p. */
+int dprb_splade_pool_fwd(const void* x, int64_t ldx, const void* W, int64_t ldw, const float* bias, const int32_t* off,
+                         int64_t T, int N, int V, int K, float* out, int64_t ldo, dprb_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Cross-encoder sequence-classification head (reranking: dpr_scale/models/citadel_models/cross_encoder.py:21-26,
  * AutoModelForSequenceClassification under no_grad).  The caller runs the head's dense layer first, on the CLS rows
