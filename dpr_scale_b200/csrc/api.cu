@@ -175,6 +175,14 @@ int dprb_splade_pool_fwd(const void* x, int64_t ldx, const void* W, int64_t ldw,
                          int64_t T, int N, int V, int K, float* out, int64_t ldo, dprb_stream_t stream) {
   return splade_pool_fwd(x, ldx, W, ldw, bias, off, T, N, V, K, out, ldo, S(stream));
 }
+int64_t dprb_expert_group_workspace_bytes(int N, int S_, int K) { return expert_group_workspace_bytes(N, S_, K); }
+int dprb_expert_group(const int32_t* ids, const float* w, const int32_t* mask, const int32_t* tokens, const void* reps,
+                      int64_t ldr, int N, int S_, int K, int P, int V, float threshold, int flags, int32_t* count,
+                      int32_t* out_expert, int32_t* out_seq, int32_t* out_tok, float* out_w, float* out_payload,
+                      void* workspace, int64_t workspace_bytes, dprb_stream_t stream) {
+  return expert_group(ids, w, mask, tokens, reps, ldr, N, S_, K, P, V, threshold, flags, count, out_expert, out_seq,
+                      out_tok, out_w, out_payload, workspace, workspace_bytes, S(stream));
+}
 int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
                          int H, int L, dprb_stream_t stream) {
   return seqcls_head_fwd(pre, weight, bias, logits, score, N, H, L, S(stream));

@@ -120,4 +120,10 @@ int maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const 
 int splade_pool_fwd(const void* x, long long ldx, const void* W, long long ldw, const float* bias, const int32_t* off,
                     long long T, int N, int V, int K, float* out, long long ldo, cudaStream_t stream);
 
+long long expert_group_workspace_bytes(int N, int S, int K);
+int expert_group(const int32_t* ids, const float* w, const int32_t* mask, const int32_t* tokens, const void* reps,
+                 long long ldr, int N, int S, int K, int P, int V, float threshold, int flags, int32_t* count,
+                 int32_t* out_expert, int32_t* out_seq, int32_t* out_tok, float* out_w, float* out_payload,
+                 void* workspace, long long workspace_bytes, cudaStream_t stream);
+
 }  // namespace dprb

@@ -8,6 +8,7 @@ one contiguous, unpadded slice of the run file (ContiguousDistributedSamplerForT
 """
 from ..transforms.dpr_transform import maybe_add_title
 from .cross_encoder import TRECDataset
+from .dpr import DenseRetrieverQueriesDataModule as _QueriesDataModule
 from .dpr import _EncodeOnlyDataModule
 
 
@@ -32,3 +33,19 @@ class DenseRetrieverRerankDataModule(_EncodeOnlyDataModule):
                                        for row in batch])
         return {"qid": [row["qid"] for row in batch], "ctx_id": [row["ctx_id"] for row in batch],
                 "query_ids": question_tensors, "contexts_ids": ctx_tensors}
+
+
+class DenseRetrieverQueriesDataModule(_QueriesDataModule):
+    """Question file for multi-vector query embedding generation (the reference's
+    ``dpr_scale.datamodule.citadel.DenseRetrieverQueriesDataModule``, datamodule/citadel.py:138-196): the readers and
+    contiguous shards of the dense one, and the reference's collate: ``query_ids`` and ``question``, plus ``topic_ids``
+    when the rows have ids (``trec_format``) and ``answers`` when they have answers."""
+
+    def collate(self, batch, stage):
+        inputs = {"query_ids": self._encode([row["question"] for row in batch]),
+                  "question": [row["question"] for row in batch]}
+        if "id" in batch[0]:
+            inputs["topic_ids"] = [row["id"] for row in batch]
+        if "answers" in batch[0]:
+            inputs["answers"] = [row["answers"] for row in batch]
+        return inputs

@@ -495,3 +495,80 @@ def splade_pool(x, W, off, K, bias=None, out=None):
                                            _ptr(off), T, N, V, int(K), _ptr(out), ldo, _stream()),
           "dprb_splade_pool_fwd")
     return out
+
+
+EXPERT_GROUP_CONTEXT_ID, EXPERT_GROUP_PER_SEQUENCE = 1, 2   # include/dprb.h DPRB_EXPERT_GROUP_*
+EXPERT_GROUP_MAX_V = 1 << 24
+
+
+def expert_group_check(N, S, K, P, V, context_id=False):
+    """ValueError for the shapes dprb_expert_group refuses (P is not read in context-id mode)."""
+    if N < 1 or not 2 <= S <= MAXSIM_MAX_S:
+        raise ValueError(f"expert grouping needs N >= 1 sequences of 2 .. {MAXSIM_MAX_S} tokens (got N={N}, S={S})")
+    if not 1 <= K <= MAXSIM_MAX_EXPERTS:
+        raise ValueError(f"expert grouping needs 1 .. {MAXSIM_MAX_EXPERTS} experts per token (got {K})")
+    if N * S * K >= 1 << 31:
+        raise ValueError(f"expert grouping needs N*S*K < 2^31 entries (got {N * S * K})")
+    if not 1 <= V < EXPERT_GROUP_MAX_V:
+        raise ValueError(f"expert grouping needs a vocabulary of 1 .. 2^24 - 1 experts (got {V})")
+    if not context_id and (P % 8 or not 8 <= P <= MAXSIM_MAX_P):
+        raise ValueError(f"expert grouping needs the token dimension to be a multiple of 8 and at most {MAXSIM_MAX_P} "
+                         f"(got {P})")
+
+
+_GROUP_WS = {}
+
+
+def expert_group(reps, ids, w, mask, V, threshold=0.0, tokens=None, per_sequence=False):
+    """Kept (token, expert) entries of one encoded batch grouped by expert (include/dprb.h dprb_expert_group).
+
+    reps bf16 [N, S, P] (unit column stride, token 0 included; None in context-id mode), ids [N, S, K] (int, in
+    [0, V)), w fp32 [N, S, K], mask [N, S]; entry (n, s, k) is kept when s >= 1, mask != 0 and w > threshold.  With
+    ``tokens`` [N, S] (context-id mode) the weight test is skipped and the payload is the token id.  Entries are sorted
+    by expert id (``per_sequence``: by (n, expert id)), ties in (n, s, k) order.
+
+    Returns device tensors of the E kept entries: (expert int32 [E], seq int32 [E], token int32 [E], weight fp32 [E],
+    payload fp32 [E, P] = weight * float(rep), or fp32 [E] = float(token id)).  Reading E is the call's one host
+    synchronisation."""
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (reps, w)):
+        raise ValueError("expert grouping runs forward only: call it under torch.no_grad()")
+    if ids.dim() != 3 or w.shape != ids.shape or mask.shape != ids.shape[:2]:
+        raise ValueError(f"expert grouping needs ids and weights [N, S, K] and a mask [N, S] (got {tuple(ids.shape)}, "
+                         f"{tuple(w.shape)} and {tuple(mask.shape)})")
+    N, S, K = ids.shape
+    ctx = tokens is not None
+    if ctx:
+        if tuple(tokens.shape) != (N, S):
+            raise ValueError(f"expert grouping needs token ids [{N}, {S}] (got {tuple(tokens.shape)})")
+        P = 0
+    else:
+        if reps is None or reps.dim() != 3 or reps.shape[:2] != (N, S):
+            raise ValueError(f"expert grouping needs reps [{N}, {S}, P] (got "
+                             f"{None if reps is None else tuple(reps.shape)})")
+        P = reps.shape[2]
+    expert_group_check(N, S, K, P, V, ctx)
+    dev = ids.device
+    lib = _lib.load()
+    ids32 = ids.to(dev, torch.int32).contiguous()
+    w32 = w.to(dev, torch.float32).contiguous()
+    m32 = mask.to(dev, torch.int32).contiguous()
+    tok32 = tokens.to(dev, torch.int32).contiguous() if ctx else None
+    if not ctx:
+        assert reps.dtype == torch.bfloat16 and reps.stride(2) == 1 and reps.stride(0) == S * reps.stride(1)
+    cap = max(N * (S - 1) * K, 1)
+    count = torch.empty(1, dtype=torch.int32, device=dev)
+    expert, seq, tok = (torch.empty(cap, dtype=torch.int32, device=dev) for _ in range(3))
+    weight = torch.empty(cap, dtype=torch.float32, device=dev)
+    payload = torch.empty((cap,) if ctx else (cap, P), dtype=torch.float32, device=dev)
+    nbytes = int(lib.dprb_expert_group_workspace_bytes(N, S, K))
+    buf = _GROUP_WS.get(dev)
+    if buf is None or buf.numel() < nbytes + 256:
+        buf = _GROUP_WS[dev] = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+    off = (-buf.data_ptr()) % 256
+    flags = (EXPERT_GROUP_CONTEXT_ID if ctx else 0) | (EXPERT_GROUP_PER_SEQUENCE if per_sequence else 0)
+    check(lib.dprb_expert_group(_ptr(ids32), _ptr(w32), _ptr(m32), _ptr(tok32), None if ctx else _ptr(reps),
+                                0 if ctx else reps.stride(1), N, S, K, P, int(V), float(threshold), flags,
+                                _ptr(count), _ptr(expert), _ptr(seq), _ptr(tok), _ptr(weight), _ptr(payload),
+                                buf.data_ptr() + off, buf.numel() - off, _stream()), "dprb_expert_group")
+    E = int(count.item())
+    return expert[:E], seq[:E], tok[:E], weight[:E], payload[:E]

@@ -333,6 +333,30 @@ int dprb_maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, c
 int dprb_splade_pool_fwd(const void* x, int64_t ldx, const void* W, int64_t ldw, const float* bias, const int32_t* off,
                          int64_t T, int N, int V, int K, float* out, int64_t ldo, dprb_stream_t stream);
 
+/* COIL / CITADEL expert-index generation: the kept (token, expert) entries of one encoded batch, grouped by expert.
+ * Replaces the per-entry loops of GenerateMultiVecEmbeddingsTask / GenerateMultiVecQueryEmbeddingsTask
+ * (dpr_scale/task/citadel_eval_task.py:43-70, :95-102, :143-171).  Entry i = (n, s, k), i = (n*S + s)*K + k, is kept when
+ *   s >= 1 and mask[n, s] != 0 and w[i] > threshold        (DPRB_EXPERT_GROUP_CONTEXT_ID: the weight test is skipped)
+ * The E kept entries are written sorted by expert id (DPRB_EXPERT_GROUP_PER_SEQUENCE: by (n, expert id)), ties in
+ * (n, s, k) order, which is the reference's iteration order:
+ *   out_expert / out_seq / out_tok int32 [E] = ids[i], n, s;   out_w fp32 [E] = w[i];
+ *   out_payload fp32 [E, P] = w[i] * float(reps[n, s, :P])   (one rounding)   or, in context-id mode, fp32 [E] =
+ *   float(tokens[n, s]);   count int32 [1] = E (device).
+ * Outputs must hold the worst case N*(S-1)*K entries.  ids int32 / w fp32 [N, S, K], mask int32 [N, S], tokens int32
+ * [N, S] (context-id mode only, else may be NULL), reps bf16 [N, S, ldr] (not read in context-id mode), 16-byte aligned.
+ * ids must lie in [0, V).  workspace: >= dprb_expert_group_workspace_bytes(N, S, K) bytes, 256-byte aligned.
+ * Integer counting only: bitwise repeatable.  Requires N >= 1, N*S*K < 2^31, 1 <= K <= 8, 2 <= S <= 512, 1 <= V < 2^24
+ * and, outside context-id mode, P % 8 == 0, 8 <= P <= 1024, ldr >= P, ldr % 8 == 0 (checked before any launch, return
+ * code 1).  Enqueues a memset and 3 launches per radix pass (ceil(log2 V / 8) passes, plus ceil(log2 N / 8) per
+ * sequence) and one gather; never synchronises. */
+#define DPRB_EXPERT_GROUP_CONTEXT_ID 1
+#define DPRB_EXPERT_GROUP_PER_SEQUENCE 2
+int64_t dprb_expert_group_workspace_bytes(int N, int S, int K);
+int dprb_expert_group(const int32_t* ids, const float* w, const int32_t* mask, const int32_t* tokens, const void* reps,
+                      int64_t ldr, int N, int S, int K, int P, int V, float threshold, int flags, int32_t* count,
+                      int32_t* out_expert, int32_t* out_seq, int32_t* out_tok, float* out_w, float* out_payload,
+                      void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Cross-encoder sequence-classification head (reranking: dpr_scale/models/citadel_models/cross_encoder.py:21-26,
  * AutoModelForSequenceClassification under no_grad).  The caller runs the head's dense layer first, on the CLS rows
