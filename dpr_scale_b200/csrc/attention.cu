@@ -36,13 +36,12 @@ int attn_bwd_lse(const void* qkv, const int32_t* attn_mask, const void* ctx, con
                  unsigned long long site_seed, cudaStream_t stream) {
   if (int rc = check_shape(nseq, S, heads, "attn_bwd")) return rc;
   if (nseq == 0) return 0;
-  if (S > SHORT_MAX) {
-    // D = rowsum(dO * ctx) in fp32
-    if (int rc = attn_bwd_long(qkv, attn_mask, ctx, lse, dctx, dqkv, nseq, S, heads, dropout_p, site_seed, stream)) return rc;
-  } else {
-    // D = rowsum(P * dP) is rebuilt in fp32 from Q, K, V, dO and lse; ctx is not read
-    if (int rc = attn_bwd_wg(qkv, attn_mask, lse, dctx, dqkv, nseq, S, heads, dropout_p, site_seed, stream)) return rc;
-  }
+  // D = rowsum(P * dP) is rebuilt in fp32 from Q, K, V, dO and lse; ctx is not read.  The S <= 128 kernel sums the
+  // QKV bias gradient itself.
+  if (S <= SHORT_MAX)
+    return attn_bwd_wg(qkv, attn_mask, lse, dctx, dqkv, dbias, nseq, S, heads, dropout_p, site_seed, stream);
+  // D = rowsum(dO * ctx) in fp32
+  if (int rc = attn_bwd_long(qkv, attn_mask, ctx, lse, dctx, dqkv, nseq, S, heads, dropout_p, site_seed, stream)) return rc;
   // the QKV bias gradient: column sums of the bf16 dQ / dK / dV
   if (dbias != nullptr) return colsum_bf16(dqkv, 3LL * heads * DH, dbias, nseq * S, 3 * heads * DH, stream);
   return 0;

@@ -61,8 +61,9 @@ int attn_bwd_lse(const void* qkv, const int32_t* attn_mask, const void* ctx, con
 
 int attn_fwd_wg(const void* qkv, const int32_t* attn_mask, void* ctx, float* lse, int nseq, int S, int heads,
                 float dropout_p, unsigned long long site_seed, cudaStream_t stream);
+// adds the QKV bias gradient into dbias when it is given
 int attn_bwd_wg(const void* qkv, const int32_t* attn_mask, const float* lse, const void* dctx,
-                void* dqkv, int nseq, int S, int heads, float dropout_p, unsigned long long site_seed,
+                void* dqkv, float* dbias, int nseq, int S, int heads, float dropout_p, unsigned long long site_seed,
                 cudaStream_t stream);
 
 int attn_cls_fwd(const void* qkv, const int32_t* attn_mask, void* ctx_cls, float* probs, int nseq, int S, int heads,
