@@ -99,6 +99,10 @@ SIGNATURES = {
     "dprb_search_topk": (c_int, [_P, _P, c_int, c_int64, c_int64, c_int, c_int, c_int64, _P, _P, _P, c_int64, _P]),
     "dprb_topk_merge_workspace_bytes": (c_int64, [c_int64, c_int]),
     "dprb_topk_merge": (c_int, [_P, _P, c_int64, c_int, c_int, _P, _P, _P, c_int64, _P]),
+    "dprb_expert_search_block_queries": (c_int, [c_int64]),
+    "dprb_expert_search_workspace_bytes": (c_int64, [c_int64, c_int]),
+    "dprb_expert_search": (c_int, [_P, _P, _P, c_int64, c_int, c_int, c_int, _P, c_int, c_int, _P, c_int64, _P, _P,
+                                   c_int64, _P, c_int, _P, _P, c_int, c_int, c_int, _P, _P, _P, c_int64, _P]),
 }
 
 _lib = None

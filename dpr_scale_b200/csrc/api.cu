@@ -201,4 +201,16 @@ int dprb_topk_merge(const float* scores, const int64_t* index, int64_t Q, int to
                     reinterpret_cast<long long*>(out_index), workspace, workspace_bytes, S(stream));
 }
 
+int dprb_expert_search_block_queries(int64_t N) { return expert_search_block_queries(N); }
+int64_t dprb_expert_search_workspace_bytes(int64_t N, int Qb) { return expert_search_workspace_bytes(N, Qb); }
+int dprb_expert_search(const void* payload, const int32_t* row, const int32_t* tile_bounds, int64_t E, int T, int P,
+                       int ldp, const void* cls, int Pc, int ldc, const int64_t* row_ids, int64_t N,
+                       const void* q_payload, const int32_t* q_seq, int64_t Eq, const void* q_cls, int Qb,
+                       const int32_t* groups, const int32_t* item_end, int G, int items, int k, float* out_scores,
+                       int64_t* out_ids, void* workspace, int64_t workspace_bytes, dprb_stream_t stream) {
+  return expert_search(payload, row, tile_bounds, E, T, P, ldp, cls, Pc, ldc, reinterpret_cast<const long long*>(row_ids),
+                       N, q_payload, q_seq, Eq, q_cls, Qb, groups, item_end, G, items, k, out_scores,
+                       reinterpret_cast<long long*>(out_ids), workspace, workspace_bytes, S(stream));
+}
+
 }  // extern "C"

@@ -127,4 +127,12 @@ int expert_group(const int32_t* ids, const float* w, const int32_t* mask, const 
                  int32_t* out_expert, int32_t* out_seq, int32_t* out_tok, float* out_w, float* out_payload,
                  void* workspace, long long workspace_bytes, cudaStream_t stream);
 
+int expert_search_block_queries(long long N);
+long long expert_search_workspace_bytes(long long N, int Qb);
+int expert_search(const void* payload, const int32_t* row, const int32_t* tile_bounds, long long E, int T, int P,
+                  int ldp, const void* cls, int Pc, int ldc, const long long* row_ids, long long N,
+                  const void* q_payload, const int32_t* q_seq, long long Eq, const void* q_cls, int Qb,
+                  const int32_t* groups, const int32_t* item_end, int G, int items, int k, float* out_scores,
+                  long long* out_ids, void* workspace, long long workspace_bytes, cudaStream_t stream);
+
 }  // namespace dprb

@@ -5,6 +5,7 @@ hand-written sm_90a kernels from libdprb.so; nothing falls back to torch math.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -572,3 +573,123 @@ def expert_group(reps, ids, w, mask, V, threshold=0.0, tokens=None, per_sequence
                                 buf.data_ptr() + off, buf.numel() - off, _stream()), "dprb_expert_group")
     E = int(count.item())
     return expert[:E], seq[:E], tok[:E], weight[:E], payload[:E]
+
+
+EXPERT_SEARCH_MAX_P = 1024        # include/dprb.h dprb_expert_search: P, Pc multiples of 8, 8 .. 1024
+EXPERT_SEARCH_MAX_K = 1024
+EXPERT_SEARCH_GROUP = 64          # query rows per work group (the kernel's wgmma M)
+EXPERT_SEARCH_CLS_TILE = 128      # CLS rows per CLS tile (the kernel's wgmma N)
+EXPERT_SEARCH_TILE_WINDOW = 112   # an index tile holds the runs that start in one 112-entry window of its expert
+EXPERT_SEARCH_TERM_LIMIT = 2.0 ** 30   # bound on a query's sum of |terms| (int64 fixed point at 2^-32)
+FP16_MAX = 65504.0
+
+
+def expert_search_check(P, Pc, V, E, N, k):
+    """ValueError for the shapes dprb_expert_search refuses (Pc None: no CLS term)."""
+    for name, w in (("payload", P), ("CLS", Pc)):
+        if w is not None and (w % 8 or not 8 <= w <= EXPERT_SEARCH_MAX_P):
+            raise ValueError(f"expert search needs the {name} width to be a multiple of 8 in 8 .. "
+                             f"{EXPERT_SEARCH_MAX_P} (got {w})")
+    if not 1 <= V < EXPERT_GROUP_MAX_V:
+        raise ValueError(f"expert search needs a vocabulary of 1 .. 2^24 - 1 experts (got {V})")
+    if not 0 <= E < 1 << 31:
+        raise ValueError(f"expert search needs fewer than 2^31 index entries (got {E})")
+    if not 1 <= N < 1 << 31:
+        raise ValueError(f"expert search needs 1 .. 2^31 - 1 passages (got {N})")
+    if not 1 <= k <= min(EXPERT_SEARCH_MAX_K, N):
+        raise ValueError(f"expert search needs 1 <= topk <= min({EXPERT_SEARCH_MAX_K}, passages={N}) (got {k})")
+
+
+def expert_search_block_queries(N):
+    """Queries per search block: the [Qb, N] int64 accumulator stays within the library's fixed 2 GiB budget."""
+    return int(_lib.load().dprb_expert_search_block_queries(int(N)))
+
+
+def expert_search_tiles(expert, row, V, window=EXPERT_SEARCH_TILE_WINDOW):
+    """Index tiles of entries sorted by (expert, row) (host int arrays [E]): (tile_bounds int32 [T + 1], tile_ptr int64
+    [V + 1] = each expert's first tile).  A tile is the runs (one row's entries of one expert) that start in the same
+    ``window``-entry window of their expert, so no run is split and a run longer than a tile stays whole."""
+    expert = np.asarray(expert, dtype=np.int64)
+    row = np.asarray(row, dtype=np.int64)
+    E = expert.size
+    if E == 0:
+        return np.zeros(1, np.int32), np.zeros(V + 1, np.int64)
+    ptr = np.zeros(V + 1, np.int64)
+    np.cumsum(np.bincount(expert, minlength=V), out=ptr[1:])
+    rs = np.flatnonzero(np.r_[True, (expert[1:] != expert[:-1]) | (row[1:] != row[:-1])])
+    ex = expert[rs]
+    win = (rs - ptr[ex]) // window
+    starts = rs[np.r_[True, (ex[1:] != ex[:-1]) | (win[1:] != win[:-1])]]
+    tile_ptr = np.zeros(V + 1, np.int64)
+    np.cumsum(np.bincount(expert[starts], minlength=V), out=tile_ptr[1:])
+    return np.r_[starts, E].astype(np.int32), tile_ptr
+
+
+def expert_search_groups(q_expert, tile_ptr, n_cls, N):
+    """Work groups of one query block: query entries sorted by expert (host int [Eq]) cut into runs of <= 64 of one
+    expert, each with its expert's tiles (experts without postings are dropped), then ``n_cls`` queries' CLS rows in
+    groups of 64 with the ceil(N / 128) CLS tiles.  Returns (groups int32 [G, 4], item_end int32 [G], items)."""
+    q_expert = np.asarray(q_expert, dtype=np.int64)
+    V = tile_ptr.size - 1
+    parts = []
+    if q_expert.size:
+        starts = np.flatnonzero(np.r_[True, q_expert[1:] != q_expert[:-1]])
+        counts = np.diff(np.r_[starts, q_expert.size])
+        xs = q_expert[starts]
+        known = xs < V
+        ntiles = np.zeros(xs.size, np.int64)
+        ntiles[known] = tile_ptr[xs[known] + 1] - tile_ptr[xs[known]]
+        ng = (counts + EXPERT_SEARCH_GROUP - 1) // EXPERT_SEARCH_GROUP
+        gi = np.repeat(np.arange(xs.size), ng)
+        j = np.arange(gi.size) - np.repeat(np.cumsum(ng) - ng, ng)
+        lo = starts[gi] + EXPERT_SEARCH_GROUP * j
+        rows = np.minimum(EXPERT_SEARCH_GROUP, counts[gi] - EXPERT_SEARCH_GROUP * j)
+        first = np.where(known[gi], tile_ptr[np.minimum(xs[gi], V - 1)], 0)
+        g = np.stack([np.zeros_like(lo), lo, rows, first, ntiles[gi]], 1)
+        parts.append(g[g[:, 4] > 0])
+    if n_cls:
+        lo = np.arange(0, n_cls, EXPERT_SEARCH_GROUP)
+        rows = np.minimum(EXPERT_SEARCH_GROUP, n_cls - lo)
+        nt = (N + EXPERT_SEARCH_CLS_TILE - 1) // EXPERT_SEARCH_CLS_TILE
+        parts.append(np.stack([np.ones_like(lo), lo, rows, np.zeros_like(lo), np.full_like(lo, nt)], 1))
+    g = np.concatenate(parts) if parts else np.zeros((0, 5), np.int64)
+    end = np.cumsum(g[:, 4])
+    items = int(end[-1]) if end.size else 0
+    if items >= 1 << 31:
+        raise ValueError(f"expert search block has {items} work items (2^31 or more): search fewer queries at once")
+    return np.ascontiguousarray(g[:, :4], dtype=np.int32), end.astype(np.int32), items
+
+
+_EXPERT_SEARCH_WS = {}
+
+
+def expert_search(payload, row, tile_bounds, P, cls, row_ids, q_payload, q_seq, q_cls, Qb, groups, item_end, items,
+                  k):
+    """One query block through dprb_expert_search (include/dprb.h).  Index: payload fp16 [E, ldp], row int32 [E],
+    tile_bounds int32 [T + 1], cls fp16 [N, ldc] or None, row_ids int64 [N] (the corpus id of each row).  Queries:
+    q_payload fp16 [Eq, ldp] sorted by expert, q_seq int32 [Eq] in [0, Qb), q_cls fp16 [Qb, ldc] or None; groups /
+    item_end / items from expert_search_groups (device int32).  Returns (scores fp32 [Qb, k], ids int64 [Qb, k])."""
+    lib = _lib.load()
+    dev = row_ids.device
+    N = row_ids.numel()
+    E, Eq = row.numel(), q_seq.numel()
+    for t in (payload, q_payload) + ((cls, q_cls) if cls is not None else ()):
+        assert t.dtype == torch.float16 and t.is_contiguous() and t.device == dev
+    assert q_payload.shape[1] == payload.shape[1]
+    Pc = 0 if cls is None else int(cls.shape[1])
+    if cls is not None:
+        assert q_cls is not None and q_cls.shape == (Qb, cls.shape[1])
+    nbytes = int(lib.dprb_expert_search_workspace_bytes(N, int(Qb)))
+    buf = _EXPERT_SEARCH_WS.get(dev)
+    if buf is None or buf.numel() < nbytes + 256:
+        _EXPERT_SEARCH_WS[dev] = None                          # free the old buffer before taking the new one
+        buf = _EXPERT_SEARCH_WS[dev] = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+    off = (-buf.data_ptr()) % 256
+    scores = torch.empty(Qb, k, dtype=torch.float32, device=dev)
+    ids = torch.empty(Qb, k, dtype=torch.int64, device=dev)
+    check(lib.dprb_expert_search(_ptr(payload), _ptr(row), _ptr(tile_bounds), E, tile_bounds.numel() - 1, int(P),
+                                 payload.shape[1], _ptr(cls), Pc, 0 if cls is None else cls.shape[1], _ptr(row_ids), N,
+                                 _ptr(q_payload), _ptr(q_seq), Eq, _ptr(q_cls), int(Qb), _ptr(groups), _ptr(item_end),
+                                 groups.shape[0], int(items), int(k), _ptr(scores), _ptr(ids), buf.data_ptr() + off,
+                                 buf.numel() - off, _stream()), "dprb_expert_search")
+    return scores, ids

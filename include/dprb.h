@@ -401,6 +401,36 @@ int64_t dprb_topk_merge_workspace_bytes(int64_t Q, int total);
 int dprb_topk_merge(const float* scores, const int64_t* index, int64_t Q, int total, int k, float* out_scores,
                     int64_t* out_index, void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * COIL / CITADEL retrieval from an expert index (the search the reference's CITADELRetrievalTask delegates to its
+ * inverted vector index, dpr_scale/task/citadel_retrieval_task.py:114).  For every query q of a block of Qb queries and
+ * every passage row d in [0, N):
+ *   score(q, d) = q_cls[q] . cls[d]                                            (only with the CLS operands)
+ *               + sum over q's entries (x, u) of max(0, max over d's entries (x, v) of u . v)    (max over {} = 0)
+ * and the k best rows per query, descending, ties towards the lower row; out_ids [Qb, k] int64 = row_ids[row] (or the
+ * row when row_ids is NULL), out_scores [Qb, k] fp32.
+ * Index: payload fp16 [E, ldp] (width P) with row int32 [E], entries sorted by expert and, within an expert, by row;
+ *   tile_bounds int32 [T + 1]: the index tiles [tile_bounds[t], tile_bounds[t+1]) partition [0, E) and never split one
+ *   row's entries of one expert; cls fp16 [N, ldc] (width Pc) or NULL.
+ * Queries: q_payload fp16 [Eq, ldp] sorted by expert, q_seq int32 [Eq] in [0, Qb); q_cls fp16 [Qb, ldc] or NULL.
+ * groups int32 [G, 4] = (section, first row, rows <= 64, first tile): section 0 = query entries [first, first + rows)
+ *   of one expert paired with that expert's tiles [first tile, first tile + n); section 1 = query CLS rows with the
+ *   ceil(N / 128) CLS tiles.  item_end int32 [G]: inclusive prefix sums of the n; items = item_end[G - 1].
+ * Products are fp32-accumulated; every term is added as int64 fixed point at 2^-32 (the caller keeps each query's sum
+ * of |terms| below 2^30), so the result is bitwise repeatable and a query's result does not depend on its block.
+ * Requires P % 8 == 0, 8 <= P <= 1024 (Pc likewise), ldp >= P and ldc >= Pc multiples of 8, 1 <= N < 2^31,
+ * E, Eq < 2^31, 1 <= k <= min(1024, N), 1 <= Qb <= dprb_expert_search_block_queries(N) (a fixed accumulator budget of
+ * 2 GiB); checked before any launch (return code 1).  workspace: >= dprb_expert_search_workspace_bytes(N, Qb) bytes,
+ * 256-byte aligned.  Enqueues two memsets and two launches; never synchronises.
+ * ------------------------------------------------------------------------------------------- */
+int dprb_expert_search_block_queries(int64_t N);
+int64_t dprb_expert_search_workspace_bytes(int64_t N, int Qb);
+int dprb_expert_search(const void* payload, const int32_t* row, const int32_t* tile_bounds, int64_t E, int T, int P,
+                       int ldp, const void* cls, int Pc, int ldc, const int64_t* row_ids, int64_t N,
+                       const void* q_payload, const int32_t* q_seq, int64_t Eq, const void* q_cls, int Qb,
+                       const int32_t* groups, const int32_t* item_end, int G, int items, int k, float* out_scores,
+                       int64_t* out_ids, void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
