@@ -81,6 +81,11 @@ SIGNATURES = {
     "dprb_sumsq_f32": (c_int, [_P, c_int64, _P, _P]),
     "dprb_adamw_step": (c_int, [_P, _P, _P, _P, _P, c_int64, c_float, c_float, c_float, c_float, c_float, c_int,
                                 c_float, _P, c_float, _P]),
+    "dprb_lamb_workspace_bytes": (c_int64, [c_int, c_int]),
+    "dprb_lamb_step": (c_int, [_P, _P, _P, _P, _P, c_int64, _P, c_int, c_int, c_float, c_float, c_float, c_float,
+                               c_float, c_float, c_int, c_int, c_int, c_float, _P, c_float, _P, c_int64, _P]),
+    "dprb_madgrad_step": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_float, c_float, c_float, c_float, c_int, c_float,
+                                  _P, c_float, _P]),
     "dprb_cast_f32_bf16": (c_int, [_P, _P, c_int64, _P]),
     "dprb_cast_bf16_f32": (c_int, [_P, _P, c_int64, _P]),
     "dprb_encoder_workspace_bytes": (c_int64, [POINTER(EncoderWeights), c_int, c_int, c_int]),

@@ -139,6 +139,21 @@ int dprb_adamw_step(float* p, const float* g, float* m, float* v, void* shadow, 
   return adamw_step(p, g, m, v, shadow, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale, sumsq,
                     max_norm, S(stream));
 }
+int64_t dprb_lamb_workspace_bytes(int nchunks, int nseg) { return lamb_workspace_bytes(nchunks, nseg); }
+int dprb_lamb_step(float* p, const float* g, float* m, float* v, void* shadow, int64_t n, const int64_t* plan,
+                   int nchunks, int nseg, float lr, float beta1, float beta2, float eps, float weight_decay,
+                   float clamp_value, int adam, int debias, int step, float grad_scale, const float* sumsq,
+                   float max_norm, void* workspace, int64_t workspace_bytes, dprb_stream_t stream) {
+  return lamb_step(p, g, m, v, shadow, n, reinterpret_cast<const long long*>(plan), nchunks, nseg, lr, beta1, beta2,
+                   eps, weight_decay, clamp_value, adam, debias, step, grad_scale, sumsq, max_norm, workspace,
+                   workspace_bytes, S(stream));
+}
+int dprb_madgrad_step(float* p, const float* g, float* grad_sum_sq, float* s, const float* x0, void* shadow, int64_t n,
+                      float lr, float momentum, float weight_decay, float eps, int k, float grad_scale,
+                      const float* sumsq, float max_norm, dprb_stream_t stream) {
+  return madgrad_step(p, g, grad_sum_sq, s, x0, shadow, n, lr, momentum, weight_decay, eps, k, grad_scale, sumsq,
+                      max_norm, S(stream));
+}
 int dprb_cast_f32_bf16(const float* src, void* dst, int64_t n, dprb_stream_t stream) {
   return cast_f32_bf16(src, dst, n, S(stream));
 }

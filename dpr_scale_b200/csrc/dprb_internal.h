@@ -92,6 +92,14 @@ int sumsq_f32(const float* g, long long n, float* out, cudaStream_t stream);
 int adamw_step(float* p, const float* g, float* m, float* v, void* shadow, long long n, float lr, float beta1,
                float beta2, float eps, float wd, int step, float grad_scale, const float* sumsq, float max_norm,
                cudaStream_t stream);
+long long lamb_workspace_bytes(int nchunks, int nseg);
+int lamb_step(float* p, const float* g, float* m, float* v, void* shadow, long long n, const long long* plan,
+              int nchunks, int nseg, float lr, float beta1, float beta2, float eps, float wd, float clamp_value,
+              int adam, int debias, int step, float grad_scale, const float* sumsq, float max_norm, void* workspace,
+              long long workspace_bytes, cudaStream_t stream);
+int madgrad_step(float* p, const float* g, float* nu, float* s, const float* x0, void* shadow, long long n, float lr,
+                 float momentum, float wd, float eps, int k, float grad_scale, const float* sumsq, float max_norm,
+                 cudaStream_t stream);
 int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t stream);
 int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t stream);
 

@@ -4,7 +4,8 @@
 //
 // Replaces torch.optim.AdamW as configured by /root/reference/dpr_scale/conf/task/optim/adamw.yaml
 // (instantiated at dpr_scale/task/dpr_task.py:124) and Lightning's gradient_clip_val
-// (conf/trainer/gpu_1_host.yaml:8 -> torch.nn.utils.clip_grad_norm_).
+// (conf/trainer/gpu_1_host.yaml:8 -> torch.nn.utils.clip_grad_norm_).  LAMB (conf/task/optim/lamb.yaml) and MADGRAD
+// (conf/task/optim/madgrad.yaml) take the same clip coefficient and refresh the shadow in the same pass.
 #include "common.cuh"
 #include "dprb_internal.h"
 
@@ -32,6 +33,18 @@ sumsq_kernel(const float* __restrict__ g, long long n, float* __restrict__ out) 
   }
 }
 
+// grad_scale * min(1, max_norm / (||grad_scale * g|| + 1e-6)): the global-norm clip, read from the device-side sum of
+// squares so no step waits on the host.
+__device__ __forceinline__ float clip_gmul(float grad_scale, const float* sumsq, float max_norm) {
+  float gmul = grad_scale;
+  if (sumsq != nullptr && max_norm > 0.f) {
+    const float total = sqrtf(*sumsq) * grad_scale;
+    const float coef = max_norm / (total + 1e-6f);
+    gmul *= fminf(coef, 1.f);
+  }
+  return gmul;
+}
+
 struct AdamArgs {
   float lr, beta1, beta2, eps, wd, bc1, bc2_rsqrt, grad_scale, max_norm;
 };
@@ -48,12 +61,7 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
 __global__ void __launch_bounds__(256)
 adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              bf16* __restrict__ shadow, long long n, AdamArgs a, const float* __restrict__ sumsq) {
-  float gmul = a.grad_scale;
-  if (sumsq != nullptr && a.max_norm > 0.f) {
-    const float total = sqrtf(*sumsq) * a.grad_scale;
-    const float coef = a.max_norm / (total + 1e-6f);
-    gmul *= fminf(coef, 1.f);
-  }
+  const float gmul = clip_gmul(a.grad_scale, sumsq, a.max_norm);
   const long long n4 = n >> 2;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 pp = reinterpret_cast<float4*>(p)[i];
@@ -107,6 +115,159 @@ uncast_kernel(const bf16* __restrict__ src, float* __restrict__ dst, long long n
   }
 }
 
+// ---------------------------------------------------------------- LAMB (torch_optimizer.Lamb 0.3.x)
+// The arena is cut into segments (one per parameter tensor) and every segment into chunks (a few thousand elements,
+// chosen by the caller) that never straddle a segment.  Pass 1 updates the moments and writes per-chunk partial sums of p^2 and
+// u^2; a second launch reduces each segment's partials in a fixed order into its trust ratio; pass 2 recomputes u from
+// the updated moments and applies it.  Every sum has one fixed order, so the update is bitwise repeatable for any grid.
+//
+// Plan (int64, built once per layout by the caller): chunk_off[C+1] | chunk_seg[C] | seg_chunk[S+1].
+struct LambArgs {
+  float beta1, beta2, eps, wd, clamp_value, step_size, grad_scale, max_norm;
+  int adam;
+};
+
+__device__ __forceinline__ float lamb_u(float p, float m, float v, const LambArgs& a) {
+  return m / (sqrtf(v) + a.eps) + a.wd * p;
+}
+
+__device__ __forceinline__ float lamb_moments(float p, float g, float& m, float& v, const LambArgs& a, float gmul) {
+  g *= gmul;
+  m = a.beta1 * m + (1.f - a.beta1) * g;
+  v = a.beta2 * v + (1.f - a.beta2) * g * g;
+  return lamb_u(p, m, v, a);
+}
+
+__global__ void __launch_bounds__(256)
+lamb_moments_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                    float* __restrict__ v, const long long* __restrict__ plan, int nchunks, LambArgs a,
+                    const float* __restrict__ sumsq, float* __restrict__ partials) {
+  __shared__ float red[2][8];
+  const float gmul = clip_gmul(a.grad_scale, sumsq, a.max_norm);
+  for (int c = blockIdx.x; c < nchunks; c += gridDim.x) {
+    const long long lo = plan[c] >> 2, hi = plan[c + 1] >> 2;
+    float pp = 0.f, uu = 0.f;
+    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+      const float4 p4 = reinterpret_cast<const float4*>(p)[i];
+      const float4 g4 = reinterpret_cast<const float4*>(g)[i];
+      float4 m4 = reinterpret_cast<float4*>(m)[i];
+      float4 v4 = reinterpret_cast<float4*>(v)[i];
+      const float ux = lamb_moments(p4.x, g4.x, m4.x, v4.x, a, gmul);
+      const float uy = lamb_moments(p4.y, g4.y, m4.y, v4.y, a, gmul);
+      const float uz = lamb_moments(p4.z, g4.z, m4.z, v4.z, a, gmul);
+      const float uw = lamb_moments(p4.w, g4.w, m4.w, v4.w, a, gmul);
+      reinterpret_cast<float4*>(m)[i] = m4;
+      reinterpret_cast<float4*>(v)[i] = v4;
+      pp += p4.x * p4.x + p4.y * p4.y + p4.z * p4.z + p4.w * p4.w;
+      uu += ux * ux + uy * uy + uz * uz + uw * uw;
+    }
+    pp = warp_sum(pp);
+    uu = warp_sum(uu);
+    if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = pp; red[1][threadIdx.x >> 5] = uu; }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+      float s = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) s += red[threadIdx.x][w];
+      partials[2 * (long long)c + threadIdx.x] = s;
+    }
+    __syncthreads();
+  }
+}
+
+// One warp per segment: trust[s] = min(||p||, clamp) / ||u|| (1 when either is 0, or in adam mode), times step_size.
+__global__ void __launch_bounds__(256)
+lamb_trust_kernel(const long long* __restrict__ plan, int nchunks, int nseg, const float* __restrict__ partials,
+                  LambArgs a, float* __restrict__ scale) {
+  const int s = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (s >= nseg) return;
+  const long long* seg_chunk = plan + 2 * (long long)nchunks + 1;
+  float pp = 0.f, uu = 0.f;
+  for (long long c = seg_chunk[s] + lane; c < seg_chunk[s + 1]; c += 32) {
+    pp += partials[2 * c];
+    uu += partials[2 * c + 1];
+  }
+  pp = warp_sum(pp);
+  uu = warp_sum(uu);
+  if (lane == 0) {
+    const float w_norm = fminf(sqrtf(pp), a.clamp_value), u_norm = sqrtf(uu);
+    const float trust = (w_norm == 0.f || u_norm == 0.f || a.adam) ? 1.f : w_norm / u_norm;
+    scale[s] = a.step_size * trust;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+lamb_apply_kernel(float* __restrict__ p, const float* __restrict__ m, const float* __restrict__ v,
+                  bf16* __restrict__ shadow, const long long* __restrict__ plan, int nchunks, LambArgs a,
+                  const float* __restrict__ scale) {
+  const long long* chunk_seg = plan + nchunks + 1;
+  for (int c = blockIdx.x; c < nchunks; c += gridDim.x) {
+    const long long lo = plan[c] >> 2, hi = plan[c + 1] >> 2;
+    const float k = scale[chunk_seg[c]];
+    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+      float4 p4 = reinterpret_cast<float4*>(p)[i];
+      const float4 m4 = reinterpret_cast<const float4*>(m)[i];
+      const float4 v4 = reinterpret_cast<const float4*>(v)[i];
+      p4.x -= k * lamb_u(p4.x, m4.x, v4.x, a);
+      p4.y -= k * lamb_u(p4.y, m4.y, v4.y, a);
+      p4.z -= k * lamb_u(p4.z, m4.z, v4.z, a);
+      p4.w -= k * lamb_u(p4.w, m4.w, v4.w, a);
+      reinterpret_cast<float4*>(p)[i] = p4;
+      if (shadow != nullptr) {
+        uint2 s2; s2.x = pack_bf16x2(p4.x, p4.y); s2.y = pack_bf16x2(p4.z, p4.w);
+        reinterpret_cast<uint2*>(shadow)[i] = s2;
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------- MADGRAD (dpr_scale/optim/madgrad.py, dense branch)
+struct MadgradArgs {
+  float lamb, eps, wd, momentum, ck, grad_scale, max_norm;
+};
+
+__device__ __forceinline__ void madgrad_one(float& p, float g, float& nu, float& s, float x0, const MadgradArgs& a,
+                                            float gmul) {
+  g *= gmul;
+  if (a.wd != 0.f) g += a.wd * p;  // coupled decay, only when set (as the reference: NaN/Inf p stays out of g)
+  if (a.momentum == 0.f) x0 = p + s / (cbrtf(nu) + a.eps);  // x0 rebuilt from the state before nu moves
+  nu += a.lamb * (g * g);
+  s += a.lamb * g;
+  const float z = x0 - s / (cbrtf(nu) + a.eps);
+  p = a.momentum == 0.f ? z : a.momentum * p + a.ck * z;
+}
+
+__global__ void __launch_bounds__(256)
+madgrad_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ nu, float* __restrict__ s,
+               const float* __restrict__ x0, bf16* __restrict__ shadow, long long n, MadgradArgs a,
+               const float* __restrict__ sumsq) {
+  const float gmul = clip_gmul(a.grad_scale, sumsq, a.max_norm);
+  const long long n4 = n >> 2;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    float4 pp = reinterpret_cast<float4*>(p)[i];
+    const float4 gg = reinterpret_cast<const float4*>(g)[i];
+    float4 nn = reinterpret_cast<float4*>(nu)[i];
+    float4 ss = reinterpret_cast<float4*>(s)[i];
+    const float4 xx = x0 != nullptr ? reinterpret_cast<const float4*>(x0)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    madgrad_one(pp.x, gg.x, nn.x, ss.x, xx.x, a, gmul); madgrad_one(pp.y, gg.y, nn.y, ss.y, xx.y, a, gmul);
+    madgrad_one(pp.z, gg.z, nn.z, ss.z, xx.z, a, gmul); madgrad_one(pp.w, gg.w, nn.w, ss.w, xx.w, a, gmul);
+    reinterpret_cast<float4*>(p)[i] = pp;
+    reinterpret_cast<float4*>(nu)[i] = nn;
+    reinterpret_cast<float4*>(s)[i] = ss;
+    if (shadow != nullptr) {
+      uint2 s2; s2.x = pack_bf16x2(pp.x, pp.y); s2.y = pack_bf16x2(pp.z, pp.w);
+      reinterpret_cast<uint2*>(shadow)[i] = s2;
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+    const long long i = (n4 << 2) + threadIdx.x;
+    float pp = p[i], nn = nu[i], ss = s[i];
+    madgrad_one(pp, g[i], nn, ss, x0 != nullptr ? x0[i] : 0.f, a, gmul);
+    p[i] = pp; nu[i] = nn; s[i] = ss;
+    if (shadow != nullptr) shadow[i] = __float2bfloat16(pp);
+  }
+}
+
 int stream_grid(long long n4, int sms) {
   long long want = (n4 + 255) / 256;
   long long cap = (long long)sms * 8;
@@ -140,6 +301,68 @@ int adamw_step(float* p, const float* g, float* m, float* v, void* shadow, long 
   a.bc2_rsqrt = 1.f / sqrtf(1.f - powf(beta2, (float)step));
   a.grad_scale = grad_scale; a.max_norm = max_norm;
   adamw_kernel<<<stream_grid(n >> 2, sms), 256, 0, stream>>>(p, g, m, v, (bf16*)shadow, n, a, sumsq);
+  DPRB_LAUNCH_CHECK();
+  return 0;
+}
+
+long long lamb_workspace_bytes(int nchunks, int nseg) {
+  if (nchunks < 1 || nseg < 1) return -1;
+  return ((2LL * nchunks + nseg) * (long long)sizeof(float) + 255) & ~255LL;
+}
+
+int lamb_step(float* p, const float* g, float* m, float* v, void* shadow, long long n, const long long* plan,
+              int nchunks, int nseg, float lr, float beta1, float beta2, float eps, float wd, float clamp_value,
+              int adam, int debias, int step, float grad_scale, const float* sumsq, float max_norm, void* workspace,
+              long long workspace_bytes, cudaStream_t stream) {
+  DPRB_REQUIRE(step >= 1, "lamb_step: step must start at 1 (got %d)", step);
+  DPRB_REQUIRE(n >= 0 && (n & 3) == 0, "lamb_step: arena length must be a multiple of 4 (got %lld)", n);
+  DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+                 reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(shadow) & 7) == 0 && (reinterpret_cast<uintptr_t>(plan) & 7) == 0,
+               "lamb_step: arenas must be 16-byte aligned");
+  if (n == 0) return 0;
+  DPRB_REQUIRE(plan != nullptr && nchunks >= nseg && nseg >= 1, "lamb_step: need a plan with 1 <= nseg <= nchunks "
+               "(got nchunks %d, nseg %d)", nchunks, nseg);
+  DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= lamb_workspace_bytes(nchunks, nseg),
+               "lamb_step: workspace of %lld bytes is smaller than dprb_lamb_workspace_bytes = %lld", workspace_bytes,
+               lamb_workspace_bytes(nchunks, nseg));
+  DPRB_NUM_SMS(sms);
+  LambArgs a;
+  a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.wd = wd; a.clamp_value = clamp_value; a.adam = adam != 0;
+  a.step_size = debias ? (float)((double)lr * sqrt(1.0 - pow((double)beta2, step)) / (1.0 - pow((double)beta1, step)))
+                       : lr;
+  a.grad_scale = grad_scale; a.max_norm = max_norm;
+  float* partials = static_cast<float*>(workspace);
+  float* scale = partials + 2LL * nchunks;
+  const int grid = nchunks < sms * 8 ? nchunks : sms * 8;
+  lamb_moments_kernel<<<grid, 256, 0, stream>>>(p, g, m, v, plan, nchunks, a, sumsq, partials);
+  DPRB_LAUNCH_CHECK();
+  lamb_trust_kernel<<<(nseg + 7) / 8, 256, 0, stream>>>(plan, nchunks, nseg, partials, a, scale);
+  DPRB_LAUNCH_CHECK();
+  lamb_apply_kernel<<<grid, 256, 0, stream>>>(p, m, v, (bf16*)shadow, plan, nchunks, a, scale);
+  DPRB_LAUNCH_CHECK();
+  return 0;
+}
+
+int madgrad_step(float* p, const float* g, float* nu, float* s, const float* x0, void* shadow, long long n, float lr,
+                 float momentum, float wd, float eps, int k, float grad_scale, const float* sumsq, float max_norm,
+                 cudaStream_t stream) {
+  DPRB_REQUIRE(k >= 0, "madgrad_step: k counts steps from 0 (got %d)", k);
+  DPRB_REQUIRE(momentum >= 0.f && momentum < 1.f, "madgrad_step: momentum must be in [0, 1) (got %g)", momentum);
+  DPRB_REQUIRE((momentum == 0.f) == (x0 == nullptr), "madgrad_step: x0 is required exactly when momentum != 0");
+  DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(nu) |
+                 reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(x0)) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(shadow) & 7) == 0,
+               "madgrad_step: arenas must be 16-byte aligned");
+  if (n == 0) return 0;
+  DPRB_NUM_SMS(sms);
+  MadgradArgs a;
+  const double lr_eff = (double)lr + (double)eps;  // the reference adds eps to the group lr
+  a.lamb = (float)(lr_eff * sqrt((double)k + 1.0));
+  a.eps = eps; a.wd = wd; a.momentum = momentum;
+  a.ck = (float)(1.0 - (double)momentum);
+  a.grad_scale = grad_scale; a.max_norm = max_norm;
+  madgrad_kernel<<<stream_grid(n >> 2, sms), 256, 0, stream>>>(p, g, nu, s, x0, (bf16*)shadow, n, a, sumsq);
   DPRB_LAUNCH_CHECK();
   return 0;
 }

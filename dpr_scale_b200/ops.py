@@ -267,6 +267,54 @@ def adamw_step(p, g, m, v, shadow, lr, beta1, beta2, eps, weight_decay, step, gr
           "dprb_adamw_step")
 
 
+LAMB_CHUNK = 8192  # elements per partial sum of the LAMB norms (32 KiB of fp32); a multiple of 4
+
+
+class LambPlan:
+    """Device-side chunk plan + workspace of dprb_lamb_step for one arena cut into contiguous segments of `seg_sizes`
+    elements (one per parameter tensor).  Built once per layout; chunks never straddle a segment."""
+
+    def __init__(self, seg_sizes, device, chunk=LAMB_CHUNK):
+        sizes = np.asarray(list(seg_sizes), dtype=np.int64)
+        if sizes.ndim != 1 or sizes.size == 0 or (sizes <= 0).any() or (sizes % 4).any() or chunk % 4:
+            raise ValueError("LambPlan: segments must be non-empty and multiples of 4 elements")
+        per = (sizes + chunk - 1) // chunk
+        seg_chunk = np.concatenate([[0], np.cumsum(per)])
+        chunk_seg = np.repeat(np.arange(sizes.size, dtype=np.int64), per)
+        seg_start = np.concatenate([[0], np.cumsum(sizes)])
+        within = np.arange(int(seg_chunk[-1]), dtype=np.int64) - seg_chunk[chunk_seg]
+        chunk_off = np.append(seg_start[chunk_seg] + within * chunk, seg_start[-1])
+        self.numel = int(seg_start[-1])
+        self.nchunks, self.nseg = int(seg_chunk[-1]), int(sizes.size)
+        self.plan = torch.from_numpy(np.concatenate([chunk_off, chunk_seg, seg_chunk])).to(device)
+        nbytes = int(_lib.load().dprb_lamb_workspace_bytes(self.nchunks, self.nseg))
+        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=device)
+
+    def trust_scale(self):
+        """step_size * trust ratio per segment as written by the last dprb_lamb_step with this plan."""
+        return self.workspace[:4 * (2 * self.nchunks + self.nseg)].view(torch.float32)[2 * self.nchunks:]
+
+
+def lamb_step(p, g, m, v, shadow, plan, lr, beta1, beta2, eps, weight_decay, clamp_value, adam, debias, step,
+              grad_scale=1.0, sumsq_buf=None, max_norm=0.0):
+    if p.numel() != plan.numel:
+        raise ValueError(f"lamb_step: arena has {p.numel()} elements, the plan covers {plan.numel}")
+    check(_lib.load().dprb_lamb_step(_ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(shadow), p.numel(), _ptr(plan.plan),
+                                     plan.nchunks, plan.nseg, float(lr), float(beta1), float(beta2), float(eps),
+                                     float(weight_decay), float(clamp_value), int(bool(adam)), int(bool(debias)),
+                                     int(step), float(grad_scale), _ptr(sumsq_buf), float(max_norm),
+                                     _ptr(plan.workspace), plan.workspace.numel(), _stream()),
+          "dprb_lamb_step")
+
+
+def madgrad_step(p, g, grad_sum_sq, s, x0, shadow, lr, momentum, weight_decay, eps, k, grad_scale=1.0, sumsq_buf=None,
+                 max_norm=0.0):
+    check(_lib.load().dprb_madgrad_step(_ptr(p), _ptr(g), _ptr(grad_sum_sq), _ptr(s), _ptr(x0), _ptr(shadow),
+                                        p.numel(), float(lr), float(momentum), float(weight_decay), float(eps), int(k),
+                                        float(grad_scale), _ptr(sumsq_buf), float(max_norm), _stream()),
+          "dprb_madgrad_step")
+
+
 def cast_f32_bf16(src, dst):
     check(_lib.load().dprb_cast_f32_bf16(_ptr(src), _ptr(dst), src.numel(), _stream()), "dprb_cast_f32_bf16")
     return dst

@@ -212,6 +212,28 @@ int dprb_sumsq_f32(const float* g, int64_t n, float* out, dprb_stream_t stream);
 int dprb_adamw_step(float* p, const float* g, float* m, float* v, void* shadow_bf16, int64_t n, float lr,
                     float beta1, float beta2, float eps, float weight_decay, int step, float grad_scale,
                     const float* sumsq, float max_norm, dprb_stream_t stream);
+/* LAMB (torch_optimizer.Lamb 0.3.x, conf/task/optim/lamb.yaml) with the same clip coefficient, per parameter tensor.
+ * With g = coef * grad_scale * grad:  m, v as Adam (no bias correction);  u = m / (sqrt(v) + eps) + weight_decay * p;
+ * trust = min(||p||, clamp_value) / ||u|| per segment (1 if either norm is 0 or adam != 0);
+ * p -= lr * (debias ? sqrt(1 - beta2^step) / (1 - beta1^step) : 1) * trust * u.  grads are read only.
+ * plan (device, int64): chunk_off[nchunks+1] | chunk_seg[nchunks] | seg_chunk[nseg+1] - chunks are contiguous ranges of
+ * the arena, every offset a multiple of 4, none straddling a segment; chunk_off[0] = 0, chunk_off[nchunks] = n.
+ * Norms are reduced per chunk and then per segment in a fixed order (no atomics): the update is bitwise repeatable.
+ * workspace: at least dprb_lamb_workspace_bytes(nchunks, nseg) bytes, 16-byte aligned (partial sums, trust ratios). */
+int64_t dprb_lamb_workspace_bytes(int nchunks, int nseg);
+int dprb_lamb_step(float* p, const float* g, float* m, float* v, void* shadow_bf16, int64_t n, const int64_t* plan,
+                   int nchunks, int nseg, float lr, float beta1, float beta2, float eps, float weight_decay,
+                   float clamp_value, int adam, int debias, int step, float grad_scale, const float* sumsq,
+                   float max_norm, void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
+/* MADGRAD, the dense branch of dpr_scale/optim/madgrad.py (conf/task/optim/madgrad.yaml), same clip coefficient.
+ * lamb = (lr + eps) * sqrt(k + 1), k counting steps from 0;  g = coef * grad_scale * grad + weight_decay * p;
+ * momentum == 0: x0 = p + s / (cbrt(grad_sum_sq) + eps) before the update (x0 must be NULL);
+ * momentum != 0: x0 is the caller's copy of the parameters taken when the optimizer was built;
+ * grad_sum_sq += lamb * g^2;  s += lamb * g;  z = x0 - s / (cbrt(grad_sum_sq) + eps);
+ * p = momentum == 0 ? z : momentum * p + (1 - momentum) * z.  grads are read only. */
+int dprb_madgrad_step(float* p, const float* g, float* grad_sum_sq, float* s, const float* x0, void* shadow_bf16,
+                      int64_t n, float lr, float momentum, float weight_decay, float eps, int k, float grad_scale,
+                      const float* sumsq, float max_norm, dprb_stream_t stream);
 /* fp32 -> bf16 shadow refresh (after a state_dict load). */
 int dprb_cast_f32_bf16(const float* src, void* dst_bf16, int64_t n, dprb_stream_t stream);
 /* bf16 -> fp32: unpacks a bf16-compressed gradient slice after its all-reduce (the `fp16_grads` path:
