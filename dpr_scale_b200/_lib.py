@@ -69,10 +69,6 @@ SIGNATURES = {
     "dprb_attn_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint64, _P]),
     "dprb_attn_cls_fwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint64, _P]),
     "dprb_attn_cls_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint64, _P]),
-    "dprb_score_ce_fwd": (c_int, [_P, _P, _P, _P, _P, c_float, _P, _P, _P, c_int, c_int, c_int, _P]),
-    "dprb_score_ce_bwd": (c_int, [_P, _P, _P, _P, _P, c_float, c_float, _P, _P, c_int, c_int, c_int, c_int,
-                                  c_int, c_int, c_int, _P]),
-    "dprb_score_tc_supported": (c_int, [c_int, c_int, c_int]),
     "dprb_score_tc_workspace_bytes": (c_int64, [c_int, c_int, c_int, c_int, c_int]),
     "dprb_score_tc_fwd": (c_int, [_P, _P, _P, _P, _P, c_float, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_int64,
                                   _P]),

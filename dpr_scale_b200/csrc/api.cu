@@ -103,18 +103,6 @@ int dprb_attn_cls_bwd(const void* qkv, const float* probs, const void* dctx_cls,
                       int heads, float dropout_p, uint64_t dropout_site_seed, dprb_stream_t stream) {
   return attn_cls_bwd(qkv, probs, dctx_cls, dqkv, nseq, Sq, heads, dropout_p, dropout_site_seed, S(stream));
 }
-int dprb_score_ce_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
-                      const int64_t* labels, float inv_temperature, float* lse, float* loss_sum, float* logits,
-                      int Q, int C, int d, dprb_stream_t stream) {
-  return score_ce_fwd(q, c, col_mask, pair_mask, labels, inv_temperature, lse, loss_sum, logits, Q, C, d, S(stream));
-}
-int dprb_score_ce_bwd(const float* q, const float* c, const float* logits, const int64_t* labels,
-                      const float* lse, float grad_scale, float inv_temperature, float* dq, float* dc, int Q,
-                      int C, int d, int q0, int nq, int c0, int nc, dprb_stream_t stream) {
-  return score_ce_bwd(q, c, logits, labels, lse, grad_scale, inv_temperature, dq, dc, Q, C, d, q0, nq, c0, nc,
-                      S(stream));
-}
-int dprb_score_tc_supported(int Q, int C, int d) { return score_tc_supported(Q, C, d) ? 1 : 0; }
 int64_t dprb_score_tc_workspace_bytes(int Q, int C, int d, int nq, int nc) {
   return score_tc_workspace_bytes(Q, C, d, nq, nc);
 }

@@ -72,14 +72,6 @@ int attn_cls_bwd(const void* qkv, const float* probs, const void* dctx_cls, void
                  float dropout_p, unsigned long long site_seed, cudaStream_t stream);
 int add_rows_bf16(void* dst, const void* src, int nrows, int H, long long stride_rows, cudaStream_t stream);
 
-int score_ce_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
-                 const int64_t* labels, float inv_t, float* lse, float* loss_sum, float* logits, int Q, int C, int d,
-                 cudaStream_t stream);
-int score_ce_bwd(const float* q, const float* c, const float* logits, const int64_t* labels, const float* lse,
-                 float grad_scale, float inv_t, float* dq, float* dc, int Q, int C, int d, int q0, int nq, int c0,
-                 int nc, cudaStream_t stream);
-
-bool score_tc_supported(int Q, int C, int d);
 long long score_tc_workspace_bytes(int Q, int C, int d, int nq, int nc);
 int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
                  const int64_t* labels, float inv_t, float* lse, float* loss_sum, float* logits, int Q, int C, int d,

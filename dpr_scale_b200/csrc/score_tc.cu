@@ -396,8 +396,6 @@ int grid_for(long long n4, int sms) {
 
 }  // namespace
 
-bool score_tc_supported(int Q, int C, int d) { return Q > 0 && C > 0 && d > 0 && d % 8 == 0; }
-
 long long score_tc_workspace_bytes(int Q, int C, int d, int nq, int nc) {
   return plan(nullptr, Q, C, d, nq < 0 ? Q : nq, nc < 0 ? C : nc).bytes;
 }
@@ -405,7 +403,9 @@ long long score_tc_workspace_bytes(int Q, int C, int d, int nq, int nc) {
 int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
                  const int64_t* labels, float inv_t, float* lse, float* loss_sum, float* logits, int Q, int C, int d,
                  int nq, int nc, void* workspace, long long workspace_bytes, cudaStream_t stream) {
-  DPRB_REQUIRE(score_tc_supported(Q, C, d), "score_tc_fwd: unsupported shape Q=%d C=%d d=%d (d %% 8 != 0)", Q, C, d);
+  DPRB_REQUIRE(Q >= 0 && C > 0 && d > 0, "score_tc_fwd: bad shape Q=%d C=%d d=%d", Q, C, d);
+  DPRB_REQUIRE(d % 8 == 0, "score_tc_fwd: d=%d must be a multiple of 8 (16-byte rows for TMA)", d);
+  if (Q == 0) return 0;
   DPRB_REQUIRE(lse != nullptr, "score_tc_fwd: lse output required");
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(c)) & 15) == 0, "score_tc_fwd: q / c must be 16-byte aligned");
   ScoreWs w = plan(workspace, Q, C, d, nq < 0 ? Q : nq, nc < 0 ? C : nc);
@@ -437,7 +437,8 @@ int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
 int score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const int64_t* labels, const float* lse,
                  float grad_scale, float inv_t, float* dq, float* dc, int Q, int C, int d, int q0, int nq, int c0, int nc,
                  void* workspace, long long workspace_bytes, cudaStream_t stream) {
-  DPRB_REQUIRE(score_tc_supported(Q, C, d), "score_tc_bwd: unsupported shape");
+  DPRB_REQUIRE(Q > 0 && C > 0 && d > 0, "score_tc_bwd: bad shape Q=%d C=%d d=%d", Q, C, d);
+  DPRB_REQUIRE(d % 8 == 0, "score_tc_bwd: d=%d must be a multiple of 8 (16-byte rows for TMA)", d);
   DPRB_REQUIRE(q0 >= 0 && nq >= 0 && q0 + nq <= Q && c0 >= 0 && nc >= 0 && c0 + nc <= C,
                "score_tc_bwd: local ranges out of bounds (q0=%d nq=%d c0=%d nc=%d)", q0, nq, c0, nc);
   ScoreWs w = plan(workspace, Q, C, d, nq, nc);

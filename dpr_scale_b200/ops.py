@@ -170,7 +170,7 @@ def attn_cls_bwd(qkv, probs, dctx_cls, nseq, S, heads, dropout_p=0.0, site_seed=
 
 
 class ScoreCtx:
-    """What the tensor-core scoring forward leaves for its backward: the workspace holding the exact bf16 operand splits
+    """What the tensor-core scoring forward leaves for its backward: the workspace holding the bf16 operand splits
     (and room for the recomputed W tiles), plus the masks / labels / lse the recomputation needs."""
 
     __slots__ = ("ws", "col_mask", "pair_mask", "labels", "lse", "shape", "local")
@@ -180,32 +180,30 @@ class ScoreCtx:
         self.shape, self.local = shape, local
 
 
-def score_tc_supported(Q, C, d):
-    return bool(_lib.load().dprb_score_tc_supported(Q, C, d))
+def _round_up8(d):
+    return (d + 7) // 8 * 8
 
 
 def score_fwd(q, c, col_mask, labels, inv_temperature, want_logits=False, pair_mask=None, local=None):
     """Fused scoring + CE forward.  Returns (loss_sum[1], lse[Q], logits or None, ctx): `ctx` (ScoreCtx) is what
-    score_bwd needs on the tensor-core path, or None when the shape falls back to the FFMA kernels (d % 8 != 0), in
-    which case logits are always produced (that backward reads them).  local = (nq, nc) sizes backward's W tiles."""
+    score_bwd needs.  local = (nq, nc) sizes backward's W tiles.  The kernels take d % 8 == 0; other widths are
+    zero-padded, which adds exactly 0 to every dot product."""
     Q, d = q.shape
     C = c.shape[0]
+    d8 = _round_up8(d)
+    if d8 != d:
+        q = torch.nn.functional.pad(q, (0, d8 - d))
+        c = torch.nn.functional.pad(c, (0, d8 - d))
     lib = _lib.load()
     lse = torch.empty(Q, dtype=torch.float32, device=q.device)
     loss_sum = torch.zeros(1, dtype=torch.float32, device=q.device)
-    if not score_tc_supported(Q, C, d):
-        logits = torch.empty(Q, C, dtype=torch.float32, device=q.device)
-        check(lib.dprb_score_ce_fwd(_ptr(q), _ptr(c), _ptr(col_mask), _ptr(pair_mask), _ptr(labels),
-                                    float(inv_temperature), _ptr(lse), _ptr(loss_sum), _ptr(logits), Q, C, d, _stream()),
-              "dprb_score_ce_fwd")
-        return loss_sum, lse, logits, None
     nq, nc = local if local is not None else (0, 0)
-    nbytes = lib.dprb_score_tc_workspace_bytes(Q, C, d, nq, nc)
+    nbytes = lib.dprb_score_tc_workspace_bytes(Q, C, d8, nq, nc)
     ws = torch.empty(int(nbytes) + 256, dtype=torch.uint8, device=q.device)
     off = (-ws.data_ptr()) % 256
     logits = torch.empty(Q, C, dtype=torch.float32, device=q.device) if want_logits else None
     check(lib.dprb_score_tc_fwd(_ptr(q), _ptr(c), _ptr(col_mask), _ptr(pair_mask), _ptr(labels), float(inv_temperature),
-                                _ptr(lse), _ptr(loss_sum), _ptr(logits), Q, C, d, nq, nc, ws.data_ptr() + off,
+                                _ptr(lse), _ptr(loss_sum), _ptr(logits), Q, C, d8, nq, nc, ws.data_ptr() + off,
                                 ws.numel() - off, _stream()), "dprb_score_tc_fwd")
     return loss_sum, lse, logits, ScoreCtx(ws, col_mask, pair_mask, labels, lse, (Q, C, d), (nq, nc))
 
@@ -213,45 +211,16 @@ def score_fwd(q, c, col_mask, labels, inv_temperature, want_logits=False, pair_m
 def score_bwd(ctx, grad_scale, inv_temperature, q0, nq, c0, nc):
     """dq[nq, d], dc[nc, d] of mean-over-Q CE for the rank-local rows / columns; tiles are recomputed (ScoreCtx)."""
     Q, C, d = ctx.shape
+    d8 = _round_up8(d)
     assert (nq, nc) == tuple(ctx.local), "score_fwd must be told the local (nq, nc) that backward asks for"
-    dq = torch.empty(nq, d, dtype=torch.float32, device=ctx.ws.device)
-    dc = torch.empty(nc, d, dtype=torch.float32, device=ctx.ws.device)
+    dq = torch.empty(nq, d8, dtype=torch.float32, device=ctx.ws.device)
+    dc = torch.empty(nc, d8, dtype=torch.float32, device=ctx.ws.device)
     off = (-ctx.ws.data_ptr()) % 256
     check(_lib.load().dprb_score_tc_bwd(_ptr(ctx.col_mask), _ptr(ctx.pair_mask), _ptr(ctx.labels), _ptr(ctx.lse),
-                                        float(grad_scale), float(inv_temperature), _ptr(dq), _ptr(dc), Q, C, d, q0,
+                                        float(grad_scale), float(inv_temperature), _ptr(dq), _ptr(dc), Q, C, d8, q0,
                                         nq, c0, nc, ctx.ws.data_ptr() + off, ctx.ws.numel() - off, _stream()),
           "dprb_score_tc_bwd")
-    return dq, dc
-
-
-def score_ce_fwd(q, c, col_mask, labels, inv_temperature, want_logits=True, pair_mask=None):
-    """(loss_sum, lse, logits) - the forward-only form used by sim_score / evaluation."""
-    loss_sum, lse, logits, _ = score_fwd(q, c, col_mask, labels, inv_temperature, want_logits, pair_mask)
-    return loss_sum, lse, logits
-
-
-def score_ce_fwd_legacy(q, c, col_mask, labels, inv_temperature, want_logits=True, pair_mask=None):
-    """The fp32 FFMA kernels (any d): kept for d % 8 != 0 and as the A/B reference of the tensor-core path."""
-    Q, d = q.shape
-    C = c.shape[0]
-    lse = torch.empty(Q, dtype=torch.float32, device=q.device)
-    loss_sum = torch.zeros(1, dtype=torch.float32, device=q.device)
-    logits = torch.empty(Q, C, dtype=torch.float32, device=q.device) if want_logits else None
-    check(_lib.load().dprb_score_ce_fwd(_ptr(q), _ptr(c), _ptr(col_mask), _ptr(pair_mask), _ptr(labels), float(inv_temperature),
-                                        _ptr(lse), _ptr(loss_sum), _ptr(logits), Q, C, d, _stream()),
-          "dprb_score_ce_fwd")
-    return loss_sum, lse, logits
-
-
-def score_ce_bwd(q, c, logits, labels, lse, grad_scale, inv_temperature, q0, nq, c0, nc):
-    Q, d = q.shape
-    C = c.shape[0]
-    dq = torch.empty(nq, d, dtype=torch.float32, device=q.device)
-    dc = torch.empty(nc, d, dtype=torch.float32, device=q.device)
-    check(_lib.load().dprb_score_ce_bwd(_ptr(q), _ptr(c), _ptr(logits), _ptr(labels), _ptr(lse), float(grad_scale),
-                                        float(inv_temperature), _ptr(dq), _ptr(dc), Q, C, d, q0, nq, c0, nc,
-                                        _stream()), "dprb_score_ce_bwd")
-    return dq, dc
+    return dq[:, :d], dc[:, :d]
 
 
 def sumsq(g, out):

@@ -6,8 +6,8 @@ Same constructor kwargs, same Lightning hook names (``setup``, ``training_step``
 ``forward``, ``encode_queries``, ``encode_contexts``, ``sim_score``), same metric names.  What changed:
 
   * encoders are ``dpr_scale_b200.models.hf_model.HFEncoder`` (libdprb.so kernels);
-  * ``sim_score`` + mask + temperature + CrossEntropyLoss (:98-105, :197-212) are ONE fused kernel
-    (``dprb_score_ce_fwd``) and its backward emits only the rank-local dq / dc (:163-195 semantics);
+  * ``sim_score`` + mask + temperature + CrossEntropyLoss (:98-105, :197-212) are ONE fused tensor-core pass
+    (``dprb_score_tc_fwd``) and its backward emits only the rank-local dq / dc (:163-195 semantics);
   * the four per-tensor all-gathers of :174-176 are ONE packed NCCL all-gather.
 """
 import os
@@ -23,30 +23,22 @@ from ..utils.lightning_shim import DDPShardedStrategy, DDPStrategy, LightningMod
 
 class _ScoreCE(torch.autograd.Function):
     """loss = mean_i CE(q_all @ c_all.T / T with masked columns, labels); grads only for the local slices.
-    Tensor-core path (d % 8 == 0): one fused pass, no logits in HBM, backward recomputes the local tiles.
-    Otherwise: the fp32 FFMA kernels with stored logits."""
+    One fused tensor-core pass, no logits in HBM; backward recomputes the local tiles."""
 
     phase = None   # optional utils.phase_timer.PhaseTimer (bench.py's per-phase leg)
 
     @staticmethod
     def forward(ctx, q_local, c_local, q_all, c_all, labels, col_mask, pair_mask, inv_t, q0, c0):
         nq, nc = q_local.shape[0], c_local.shape[0]
-        loss_sum, lse, logits, sctx = ops.score_fwd(q_all, c_all, col_mask, labels, inv_t, False, pair_mask, (nq, nc))
-        ctx.sctx = sctx
-        if sctx is None:
-            ctx.save_for_backward(q_all, c_all, logits, labels, lse)
+        loss_sum, _, _, ctx.sctx = ops.score_fwd(q_all, c_all, col_mask, labels, inv_t, False, pair_mask, (nq, nc))
         ctx.meta = (inv_t, q0, nq, c0, nc)
         return loss_sum[0] / q_all.shape[0]
 
     @staticmethod
     def backward(ctx, g):
         inv_t, q0, nq, c0, nc = ctx.meta
-        if ctx.sctx is not None:
-            dq, dc = ops.score_bwd(ctx.sctx, 1.0, inv_t, q0, nq, c0, nc)
-            ctx.sctx = None
-        else:
-            q_all, c_all, logits, labels, lse = ctx.saved_tensors
-            dq, dc = ops.score_ce_bwd(q_all, c_all, logits, labels, lse, 1.0, inv_t, q0, nq, c0, nc)
+        dq, dc = ops.score_bwd(ctx.sctx, 1.0, inv_t, q0, nq, c0, nc)
+        ctx.sctx = None
         dq, dc = dq * g, dc * g
         if _ScoreCE.phase is not None:
             _ScoreCE.phase.mark("score_bwd")
@@ -143,7 +135,7 @@ class DenseRetrieverTask(LightningModule):
         c = context_repr.detach().float().contiguous()
         labels = torch.zeros(q.shape[0], dtype=torch.int64, device=q.device)
         pm = None if mask is None else mask.to(q.device, torch.uint8).contiguous()
-        _, _, logits = ops.score_ce_fwd(q, c, None, labels, 1.0, True, pm)
+        _, _, logits, _ = ops.score_fwd(q, c, None, labels, 1.0, True, pm)
         return logits
 
     # ------------------------------------------------------------------ optimizer / schedule
@@ -241,7 +233,7 @@ class DenseRetrieverTask(LightningModule):
         pos_ctx_indices = batch["pos_ctx_indices"].to(dev, torch.int64)
         mask = batch["ctx_mask"].to(dev)
         query_repr, contexts_repr = self(batch["query_ids"], batch["contexts_ids"])
-        loss_sum, _, scores = ops.score_ce_fwd(query_repr.contiguous(), contexts_repr.contiguous(),
+        loss_sum, _, scores, _ = ops.score_fwd(query_repr.contiguous(), contexts_repr.contiguous(),
                                                mask.to(torch.uint8).contiguous(), pos_ctx_indices, 1.0, True)
         loss = loss_sum[0] / query_repr.shape[0]
         return (self.compute_rank_metrics(scores, pos_ctx_indices), query_repr, contexts_repr, pos_ctx_indices,
@@ -292,7 +284,7 @@ class DenseRetrieverTask(LightningModule):
                 all_c = g_c.reshape(-1, g_c.shape[-1])
                 all_m = g_m.reshape(-1)
             all_q = torch.cat(qs, 0)
-            loss_sum, _, scores = ops.score_ce_fwd(all_q.contiguous(), all_c.contiguous(),
+            loss_sum, _, scores, _ = ops.score_fwd(all_q.contiguous(), all_c.contiguous(),
                                                    all_m.to(torch.uint8).contiguous(), labels.contiguous(), 1.0, True)
             total_count = all_q.size(0)
             total_ctx_count = scores.size(1) - torch.sum(all_m)

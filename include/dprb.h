@@ -25,7 +25,7 @@ extern "C" {
 
 typedef void* dprb_stream_t; /* cudaStream_t */
 
-#define DPRB_VERSION 100
+#define DPRB_VERSION 101
 
 int dprb_version(void);
 const char* dprb_last_error(void);
@@ -166,32 +166,24 @@ int dprb_attn_cls_bwd(const void* qkv_bf16, const float* probs, const void* dctx
  * Fused in-batch-negative scoring + softmax cross-entropy.
  * Replaces dpr_scale/task/dpr_task.py:98-105 (sim_score: q @ c.T, scores[mask] = -inf),
  * :197 (mask.repeat), :211 (scores /= T), :212 (nn.CrossEntropyLoss, mean over Q).
- *   q fp32 [Q,d], c fp32 [C,d], col_mask u8 [C] (1 = dummy ctx -> -inf), labels i64 [Q];
+ *   q fp32 [Q,d], c fp32 [C,d] (16-byte aligned), col_mask u8 [C] (1 = dummy ctx -> -inf), labels i64 [Q];
  *   pair_mask u8 [Q,C] (optional, 1 -> -inf): the per-query block mask of the non-in-batch branch (:199-207).
- * Outputs: lse[Q], loss_sum (sum over rows of lse - logit[label]; caller divides by Q),
- *          logits fp32 [Q,C] (masked columns = -inf) if non-NULL; required when backward follows.
+ *   d % 8 == 0 (pad q and c with zero columns otherwise: they add exactly 0 to every product); Q == 0 is a no-op.
+ * Outputs: lse[Q], loss_sum (caller-zeroed; += sum over rows of lse - logit[label]; caller divides by Q),
+ *          logits fp32 [Q,C] (masked columns = -inf) only if non-NULL.
  * Backward of mean-over-Q loss (grad_scale = upstream dL, normally 1):
  *   dq[q0:q0+nq, :]  (rows owned by this rank)  and  dc[c0:c0+nc, :] (columns owned by this rank),
  *   reproducing dpr_task.py:163-195 where remote slices are detached constants.
- * ------------------------------------------------------------------------------------------- */
-int dprb_score_ce_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
-                      const int64_t* labels, float inv_temperature, float* lse, float* loss_sum, float* logits,
-                      int Q, int C, int d, dprb_stream_t stream);
-int dprb_score_ce_bwd(const float* q, const float* c, const float* logits, const int64_t* labels,
-                      const float* lse, float grad_scale, float inv_temperature, float* dq, float* dc, int Q,
-                      int C, int d, int q0, int nq, int c0, int nc, dprb_stream_t stream);
-
-/* The same operator on the tensor cores, in ONE pass (the form BASELINE.json's north_star names): similarity tile via
- * wgmma tiles staged in shared memory, online row max / sum-exp / label pick per row, loss accumulated by the last
- * tile of each row block; logits reach HBM only if `logits` is non-NULL.  fp32 fidelity comes from an exact 3-way bf16
- * split of q and c (six partial products per k-block, fp32 accumulate): logits agree with the fp32 product of
- * dpr_task.py:99 to ~1e-6 relative.  Backward RECOMPUTES the tiles of the rank-local row block and column block
- * (no stored logits) and runs dq = W_rows c, dc = W_cols^T q on the library's GEMM.
+ * ONE tensor-core pass (the form BASELINE.json's north_star names): similarity tile via wgmma tiles staged in shared
+ * memory, online row max / sum-exp / label pick per row, loss accumulated by the last tile of each row block.
+ * fp32 fidelity comes from a 2-part bf16 split of q and c (x ~ h + m; the three products h.m, m.h, h.h per k-block,
+ * fp32 accumulate): logits agree with the fp32 product of dpr_task.py:99 to a few 1e-6 of max|logit|.  Backward
+ * RECOMPUTES the tiles of the rank-local row block and column block (no stored logits) and runs dq = W_rows c,
+ * dc = W_cols^T q on the library's GEMM.
  *   nq / nc: the local row / column counts backward will ask for (sizes the workspace; -1 = all).
  *   workspace: caller-owned, 256-byte aligned, >= dprb_score_tc_workspace_bytes(...); it carries the operand splits
  *   from the forward call to the backward call of the same step.
- * Requires d % 8 == 0 (dprb_score_tc_supported); other shapes use dprb_score_ce_fwd/bwd above. */
-int dprb_score_tc_supported(int Q, int C, int d);
+ * ------------------------------------------------------------------------------------------- */
 int64_t dprb_score_tc_workspace_bytes(int Q, int C, int d, int nq, int nc);
 int dprb_score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
                       const int64_t* labels, float inv_temperature, float* lse, float* loss_sum, float* logits, int Q,

@@ -479,8 +479,8 @@ def check_attention(nseq=3, S=128, heads=2, masked=True, seed=4, dropout=0.0, ma
 
 # ------------------------------------------------------------------ scoring + CE
 def check_score_ce(Q=37, C=250, d=768, inv_t=2.0, q0=8, nq=16, c0=40, nc=100, seed=5, pair=False):
-    """Fused scoring + CE: the tensor-core single-pass path (d % 8 == 0; tiles recomputed in backward, no logits in HBM
-    unless asked) AND the fp32 FFMA kernels, both against oracle/task.py (dpr_task.py:98-105, :197-212)."""
+    """Fused scoring + CE on the tensor-core single pass (tiles recomputed in backward, no logits in HBM unless asked;
+    d % 8 != 0 zero-padded) against oracle/task.py (dpr_task.py:98-105, :197-212)."""
     g = torch.Generator().manual_seed(seed)
     q = torch.randn(Q, d, generator=g)
     c = torch.randn(C, d, generator=g)
@@ -511,21 +511,26 @@ def check_score_ce(Q=37, C=250, d=768, inv_t=2.0, q0=8, nq=16, c0=40, nc=100, se
         _close(tag + "dq", dq, qr.grad[q0:q0 + nq], 1e-4, 1e-6, res)
         _close(tag + "dc", dc, cr.grad[c0:c0 + nc], 1e-4, 1e-6, res)
 
-    # legacy fp32 FFMA kernels (stored logits)
-    loss_sum, lse, logits = ops.score_ce_fwd_legacy(d_(q), d_(c), d_(mask.to(torch.uint8)), d_(labels), inv_t, True, pmd)
-    dq, dc = ops.score_ce_bwd(d_(q), d_(c), logits, d_(labels), lse, 1.0, inv_t, q0, nq, c0, nc)
-    compare("ffma_", loss_sum, lse, logits, dq, dc)
-    if ops.score_tc_supported(Q, C, d):
-        # training form: no logits, backward recomputes the local tiles
-        loss_sum, lse, logits, ctx = ops.score_fwd(d_(q), d_(c), d_(mask.to(torch.uint8)), d_(labels), inv_t, False, pmd, (nq, nc))
-        assert logits is None and ctx is not None
-        dq, dc = ops.score_bwd(ctx, 1.0, inv_t, q0, nq, c0, nc)
-        compare("tc_", loss_sum, lse, None, dq, dc)
-        # evaluation form: logits requested; a second call on the same shapes (counters must have been reset)
-        loss_sum2, lse2, logits2, _ = ops.score_fwd(d_(q), d_(c), d_(mask.to(torch.uint8)), d_(labels), inv_t, True, pmd)
-        compare("tc2_", loss_sum2, lse2, logits2, dq, dc)
-        assert torch.equal(lse2, lse)
+    # training form: no logits, backward recomputes the local tiles
+    loss_sum, lse, logits, ctx = ops.score_fwd(d_(q), d_(c), d_(mask.to(torch.uint8)), d_(labels), inv_t, False, pmd, (nq, nc))
+    assert logits is None and ctx is not None
+    dq, dc = ops.score_bwd(ctx, 1.0, inv_t, q0, nq, c0, nc)
+    compare("tc_", loss_sum, lse, None, dq, dc)
+    # evaluation form: logits requested; a second call on the same shapes (counters must have been reset)
+    loss_sum2, lse2, logits2, _ = ops.score_fwd(d_(q), d_(c), d_(mask.to(torch.uint8)), d_(labels), inv_t, True, pmd)
+    compare("tc2_", loss_sum2, lse2, logits2, dq, dc)
+    assert torch.equal(lse2, lse)
     return res
+
+
+def check_score_ce_no_queries(C=33, d=128):
+    """Q = 0: the forward launches nothing and returns a zero loss sum, an empty lse and empty logits."""
+    c = torch.randn(C, d, device=DEV)
+    q = torch.empty(0, d, device=DEV)
+    labels = torch.empty(0, dtype=torch.int64, device=DEV)
+    loss_sum, lse, logits, _ = ops.score_fwd(q, c, None, labels, 1.0, True)
+    assert float(loss_sum) == 0.0 and lse.shape == (0,) and logits.shape == (0, C)
+    return {"loss_sum": float(loss_sum)}
 
 
 # ------------------------------------------------------------------ optimizer
@@ -590,7 +595,8 @@ CHECKS["score_ce_8gpu_shape"] = lambda: check_score_ce(Q=1024, C=8192, d=768, in
                                                        nc=1024, seed=16)     # cfg 3: global 1024 x 8192 scores per rank
 CHECKS["score_ce_pair_mask"] = lambda: check_score_ce(Q=130, C=300, d=128, inv_t=1.0, q0=1, nq=129, c0=0, nc=300, seed=17, pair=True)
 CHECKS["score_ce_cfg4_shape"] = lambda: check_score_ce(Q=512, C=1024, d=1024, inv_t=1.0, q0=64, nq=64, c0=0, nc=1024, seed=18)
-CHECKS["score_ce_odd_d"] = lambda: check_score_ce(Q=9, C=33, d=100, inv_t=1.0, q0=0, nq=9, c0=0, nc=33, seed=19)   # d % 8 != 0 -> FFMA only
+CHECKS["score_ce_odd_d"] = lambda: check_score_ce(Q=9, C=33, d=100, inv_t=1.0, q0=0, nq=9, c0=0, nc=33, seed=19)   # d % 8 != 0 -> zero-padded to 104
+CHECKS["score_ce_no_queries"] = lambda: check_score_ce_no_queries()
 CHECKS["score_ce_ragged_splits"] = lambda: check_score_ce(Q=70, C=1999, d=200, inv_t=0.5, q0=3, nq=60, c0=17, nc=1500,
                                                           seed=17)
 CHECKS["attn_tc_many"] = lambda: check_attention(40, 128, 12, True, seed=9)

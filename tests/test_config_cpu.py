@@ -36,7 +36,7 @@ def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(_lib.LIB_PATH)
     for name in declared:
         assert hasattr(lib, name), name
-    assert _lib.load().dprb_version() == 100
+    assert _lib.load().dprb_version() == 101
 
 
 def test_encoder_rejects_unsupported_configs_and_cpu_execution():

@@ -37,8 +37,8 @@ q.retain_grad(); c.retain_grad()
 loss = task.training_step(batch, 0)
 print("loss", float(loss), float(l_or), float(g["loss"]))
 from dpr_scale_b200 import ops
-ls, lse, logits = ops.score_ce_fwd(q.detach(), c.detach(), batch["ctx_mask"].to(torch.uint8).cuda(), batch["pos_ctx_indices"].cuda(), 1.0 / T)
-dq, dc = ops.score_ce_bwd(q.detach(), c.detach(), logits, batch["pos_ctx_indices"].cuda(), lse, 1.0, 1.0 / T, 0, 4, 0, 8)
+_, _, _, sctx = ops.score_fwd(q.detach(), c.detach(), batch["ctx_mask"].to(torch.uint8).cuda(), batch["pos_ctx_indices"].cuda(), 1.0 / T, False, None, (4, 8))
+dq, dc = ops.score_bwd(sctx, 1.0, 1.0 / T, 0, 4, 0, 8)
 print("dq vs oracle", cosine(dq.cpu(), qd.grad), rel_l2(dq.cpu(), qd.grad), "dc", cosine(dc.cpu(), cd.grad), rel_l2(dc.cpu(), cd.grad))
 loss.backward()
 torch.cuda.synchronize()

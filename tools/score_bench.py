@@ -30,10 +30,6 @@ for Q, C, nq, nc in SHAPES:
     q, c = torch.randn(Q, d, device="cuda"), torch.randn(C, d, device="cuda")
     mask = torch.zeros(C, dtype=torch.uint8, device="cuda")
     labels = torch.randint(0, C, (Q,), device="cuda")
-    loss, lse, logits = ops.score_ce_fwd_legacy(q, c, mask, labels, 1.0)
-    f = timeit(lambda: ops.score_ce_fwd_legacy(q, c, mask, labels, 1.0))
-    b = timeit(lambda: ops.score_ce_bwd(q, c, logits, labels, lse, 1.0, 1.0, 0, nq, 0, nc))
-    print(f"Q={Q} C={C} FFMA (r1): fwd {f:8.1f} us ({2.0*Q*C*d/f/1e6:6.2f} TFLOP/s)   bwd(dq {nq} rows, dc {nc} cols) {b:8.1f} us", flush=True)
     _, _, _, ctx = ops.score_fwd(q, c, mask, labels, 1.0, False, None, (nq, nc))
     f = timeit(lambda: ops.score_fwd(q, c, mask, labels, 1.0, False, None, (nq, nc)))
     b = timeit(lambda: ops.score_bwd(ctx, 1.0, 1.0, 0, nq, 0, nc))
