@@ -216,4 +216,13 @@ int dprb_expert_search(const void* payload, const int32_t* row, const int32_t* t
                        reinterpret_cast<long long*>(out_ids), workspace, workspace_bytes, S(stream));
 }
 
+int64_t dprb_sqerr_workspace_bytes(int rows, int d) {
+  (void)d;
+  return sqerr_workspace_bytes(rows);
+}
+int dprb_sqerr_fwd(const float* x, int64_t ldx, const float* t, int64_t ldt, int rows, int d, float* loss_sum, float* dx,
+                   int64_t lddx, void* workspace, int64_t workspace_bytes, dprb_stream_t stream) {
+  return sqerr_fwd(x, ldx, t, ldt, rows, d, loss_sum, dx, lddx, workspace, workspace_bytes, S(stream));
+}
+
 }  // extern "C"

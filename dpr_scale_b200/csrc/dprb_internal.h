@@ -135,4 +135,8 @@ int expert_search(const void* payload, const int32_t* row, const int32_t* tile_b
                   const int32_t* groups, const int32_t* item_end, int G, int items, int k, float* out_scores,
                   long long* out_ids, void* workspace, long long workspace_bytes, cudaStream_t stream);
 
+long long sqerr_workspace_bytes(int rows);
+int sqerr_fwd(const float* x, long long ldx, const float* t, long long ldt, int rows, int d, float* loss_sum, float* dx,
+              long long lddx, void* workspace, long long workspace_bytes, cudaStream_t stream);
+
 }  // namespace dprb

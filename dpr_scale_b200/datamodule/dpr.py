@@ -31,6 +31,7 @@ import threading
 import numpy as np
 import torch
 
+from ..transforms.dpr_distill_transform import DPRDistillTransform
 from ..transforms.dpr_transform import DPRTransform, maybe_add_title
 from ..transforms.hf_transform import HFTransform
 from ..utils.lightning_shim import LightningDataModule
@@ -381,6 +382,35 @@ class DenseRetrieverJsonlDataModule(DenseRetrieverDataModuleBase):
             return self.dpr_transform(batch, stage)
         rows = batch if type(batch) is list else batch[self.dpr_transform.text_column]
         return self.dpr_transform.finish(self.dpr_transform.select(rows, stage))
+
+
+class DPRDistillJsonlDataModule(DenseRetrieverDataModuleBase):
+    """Distillation JSONL (datamodule/dpr.py:225-266 of the reference): question + target vectors per row, assembled by
+    DPRDistillTransform on the BatchStream thread (JSON, sampling, vector parsing, one tokeniser call), staged in pinned
+    memory and copied to the GPU on the side stream.  Same keyword arguments, plus ``prefetch_batches`` (0 =
+    synchronous), ``device_prefetch`` and ``fast_tokenize``."""
+
+    def __init__(self, transform, train_path: str, val_path: str, test_path: str, batch_size: int = 2,
+                 val_batch_size: int = 0, test_batch_size: int = 0, pos_ctx_sample: bool = True, drop_last: bool = False,
+                 num_workers: int = 0, prefetch_batches: int = 4, device_prefetch: bool = True, fast_tokenize: bool = True,
+                 *args, **kwargs):
+        super().__init__(transform)
+        self.batch_size = batch_size
+        self.val_batch_size = val_batch_size if val_batch_size else batch_size
+        self.test_batch_size = test_batch_size if test_batch_size else self.val_batch_size
+        self.drboost_distill_transform = DPRDistillTransform(transform, pos_ctx_sample, **kwargs)
+        self.num_workers = num_workers     # accepted; assembly runs on the BatchStream thread
+        self.prefetch_batches = prefetch_batches
+        self.device_prefetch = device_prefetch
+        self.fast_tokenize = fast_tokenize
+        self.datasets = {"train": LineFile(train_path), "valid": LineFile(val_path), "test": LineFile(test_path)}
+
+    def collate(self, batch, stage):
+        tf = self.drboost_distill_transform
+        if not self.fast_tokenize:
+            return tf(batch, stage)
+        rows = batch if type(batch) is list else batch[tf.text_column]
+        return tf.finish(tf.select(rows, stage))
 
 
 class DenseRetrieverMultiJsonlDataModule(DenseRetrieverJsonlDataModule):

@@ -16,6 +16,13 @@ from .trainer import Trainer
 from .utils.config import compose, instantiate
 
 TASK = "dpr_scale_b200.task.dpr_eval_task.GenerateEmbeddingsTask"
+# task=drboost: the same dumps over the concatenated embeddings of the weak encoders
+DRBOOST = "dpr_scale_b200.task.drboost_task.DrBoostTask"
+DRBOOST_DUMPS = {
+    TASK: "dpr_scale_b200.task.drboost_task.DrBoostGenerateEmbeddingsTask",
+    "dpr_scale_b200.task.dpr_eval_task.GenerateQueryEmbeddingsTask":
+        "dpr_scale_b200.task.drboost_task.DrBoostGenerateQueryEmbeddingsTask",
+}
 
 
 def run(argv, target):
@@ -30,6 +37,8 @@ def run(argv, target):
     init_process_group()
     cfg = compose(name, argv)
     cfg.task.datamodule = None
+    if cfg.task._target_ == DRBOOST:
+        target = DRBOOST_DUMPS[target]
     cfg.task._target_ = target
     cfg.task.setdefault("checkpoint_path", None)
     task = instantiate(cfg.task, _recursive_=False)

@@ -223,6 +223,32 @@ def score_bwd(ctx, grad_scale, inv_temperature, q0, nq, c0, nc):
     return dq[:, :d], dc[:, :d]
 
 
+_SQERR_WS = {}
+
+
+def sqerr(x, t, want_dx=True):
+    """Squared-error sum (include/dprb.h dprb_sqerr_fwd): x, t fp32 [rows, d] with unit column stride.  Returns
+    (loss_sum fp32 [1], dx = 2 (x - t) fp32 [rows, d] or None)."""
+    if x.dim() != 2 or x.shape != t.shape:
+        raise ValueError(f"squared error needs two [rows, d] operands of one shape (got {tuple(x.shape)} and "
+                         f"{tuple(t.shape)})")
+    if x.dtype != torch.float32 or t.dtype != torch.float32:
+        raise ValueError(f"squared error needs fp32 operands (got {x.dtype} and {t.dtype})")
+    x = x if x.stride(1) == 1 else x.contiguous()
+    t = t if t.stride(1) == 1 else t.contiguous()
+    rows, d = x.shape
+    lib = _lib.load()
+    loss_sum = torch.empty(1, dtype=torch.float32, device=x.device)
+    dx = torch.empty(rows, d, dtype=torch.float32, device=x.device) if want_dx else None
+    nbytes = int(lib.dprb_sqerr_workspace_bytes(rows, d))
+    buf = _SQERR_WS.get(x.device)
+    if buf is None or buf.numel() < nbytes:
+        buf = _SQERR_WS[x.device] = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=x.device)
+    check(lib.dprb_sqerr_fwd(_ptr(x), max(x.stride(0), d), _ptr(t), max(t.stride(0), d), rows, d, _ptr(loss_sum),
+                             _ptr(dx), d, buf.data_ptr(), buf.numel(), _stream()), "dprb_sqerr_fwd")
+    return loss_sum, dx
+
+
 def sumsq(g, out):
     check(_lib.load().dprb_sumsq_f32(_ptr(g), g.numel(), _ptr(out), _stream()), "dprb_sumsq_f32")
     return out

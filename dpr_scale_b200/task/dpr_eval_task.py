@@ -39,6 +39,9 @@ class _EmbeddingDumpTask(DenseRetrieverTask):
             return
         print(f"Loading checkpoint from {self.checkpoint_path}")
         state = torch.load(self.checkpoint_path, map_location="cpu", weights_only=False)["state_dict"]
+        self._load_state(state)
+
+    def _load_state(self, state):
         self.load_state_dict(state)
 
     # -- per-batch: encode, then park the result in pinned memory without waiting for it
@@ -147,6 +150,17 @@ class GenerateQueryEmbeddingsTask(GenerateEmbeddingsTask):
         self.hnsw_index = hnsw_index
         self.output_path = output_path
         self.query_emb_output_path = query_emb_output_path or os.path.join(self.ctx_embeddings_dir, "query_reps.pkl")
+
+    def _load_state(self, state):
+        """A distillation checkpoint (task/dpr_distill_task.py) holds a query encoder only: its context encoder keys
+        may be absent.  Every other missing or unexpected key raises, as a strict load does."""
+        if any(k.startswith("context_encoder.") for k in state):
+            return self.load_state_dict(state)
+        missing, unexpected = self.load_state_dict(state, strict=False)
+        missing = [k for k in missing if not k.startswith("context_encoder.")]
+        if missing or unexpected:
+            raise RuntimeError(f"Error(s) in loading state_dict for {type(self).__name__}: missing keys {missing}, "
+                               f"unexpected keys {unexpected}")
 
     def _encode(self, query_ids):
         return self.encode_queries(query_ids)

@@ -86,7 +86,8 @@ class Trainer:
 
     def _encoders(self):
         encs, seen = [], set()
-        for e in (self.task.query_encoder, self.task.context_encoder):
+        # a distillation task trains a query encoder only
+        for e in (self.task.query_encoder, getattr(self.task, "context_encoder", self.task.query_encoder)):
             if id(e) not in seen:
                 seen.add(id(e))
                 encs.append(e)

@@ -65,6 +65,22 @@ except Exception:  # noqa
                     d[k] = v
             self.logged.update(d)
 
+        @classmethod
+        def load_from_checkpoint(cls, checkpoint_path, map_location=None, **kwargs):
+            """Rebuild the task from a checkpoint's ``hyper_parameters`` (kwargs override them), build its modules
+            through ``on_load_checkpoint`` and load the ``state_dict`` strictly - Lightning's classmethod of that name
+            for the files utils/checkpoint.ModelCheckpoint writes."""
+            ckpt = torch.load(checkpoint_path, map_location="cpu", weights_only=False)
+            if not isinstance(ckpt, dict) or "state_dict" not in ckpt:
+                raise ValueError(f"{checkpoint_path} is not a checkpoint: it has no state_dict")
+            hparams = dict(ckpt.get("hyper_parameters") or {})
+            hparams.update(kwargs)
+            model = cls(**hparams)
+            if hasattr(model, "on_load_checkpoint"):
+                model.on_load_checkpoint(ckpt)
+            model.load_state_dict(ckpt["state_dict"])
+            return model.to(map_location) if map_location is not None else model
+
         @property
         def global_rank(self):
             return dist.get_rank() if dist.is_available() and dist.is_initialized() else 0

@@ -445,6 +445,22 @@ int dprb_expert_search(const void* payload, const int32_t* row, const int32_t* t
                        const int32_t* groups, const int32_t* item_end, int G, int items, int k, float* out_scores,
                        int64_t* out_ids, void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Squared-error sum for query-encoder distillation (MSELoss(reduction="sum") of the reference's DPRDistillTask,
+ * dpr_scale/task/dpr_distill_task.py:43, :167, :186, and the gradient autograd takes through it):
+ *   loss_sum[0] = sum_{r < rows, c < d} (x[r, c] - t[r, c])^2
+ *   dx[r, c]    = 2 (x[r, c] - t[r, c])            (only when dx is not NULL; evaluation passes NULL)
+ * x, t, dx fp32 row-major with row strides ldx, ldt, lddx (elements).  dx equals fp32 2 * (x - t) bit for bit; the
+ * squares are rounded to fp32 and summed in double, per block and then over the blocks' partials in a fixed order
+ * (no atomics), so loss_sum is bitwise repeatable.  16-byte loads when d, the strides and the pointers allow them.
+ * workspace: >= dprb_sqerr_workspace_bytes(rows, d) bytes, 8-byte aligned.  Requires rows >= 0, d >= 1, strides at
+ * least d (checked before any launch, return code 1).  Enqueues two launches (one when rows == 0, which writes 0);
+ * never synchronises.
+ * ------------------------------------------------------------------------------------------- */
+int64_t dprb_sqerr_workspace_bytes(int rows, int d);
+int dprb_sqerr_fwd(const float* x, int64_t ldx, const float* t, int64_t ldt, int rows, int d, float* loss_sum, float* dx,
+                   int64_t lddx, void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
