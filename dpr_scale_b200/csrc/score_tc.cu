@@ -12,7 +12,14 @@
 // fp64 product the logits agree to a few 1e-6 of max|logit| - inside a 1e-5 |logit| + 1e-3 tolerance -
 // where the reference under AMP computes this product in fp16 (spacing 0.25 at |s| ~ 300).  (A three-part split with
 // six products was measured first: 1.5x the L2 -> shared-memory traffic, which is what bounds this kernel, for
-// accuracy nobody can observe behind the fp32 softmax.)
+// accuracy nobody can observe behind the fp32 softmax.)  tests/test_score_fitted_gpu.py measures at most 5.4e-6 of a
+// row's max |logit| for |logit| 20 ... 250 (H100 80GB HBM3, 700 W).
+//
+// Softmax in base 2 (s2 = logit * log2 e): the forward keeps, per row, the max M and L = sum_j 2^(s2_j - M) less
+// the maximum's own term 1, and writes M and lg2(1 + L) to the workspace.  loss = (M - s2_label) ln2 + log1p(L):
+// when the label is the maximum the first term is exactly 0 and the loss (down to 1e-30 in a fitted row) keeps a few
+// ulp of itself, where lse - logit[label] would be a difference of two numbers rounded at |logit|.  The backward
+// forms p = 2^((s2 - M) - lg2(1 + L)), so every row of W sums to 0 within a few ulp of 1 at any |logit|.
 //
 // Backward recomputes tiles instead of reading stored logits: one launch rebuilds W = softmax - onehot for the local
 // row block [nq x C] and the local column block [Q x nc] (bf16 hi + lo), and dq = W_rows c, dc = W_cols^T q run as
@@ -52,11 +59,10 @@ struct ScoreParams {
   float* lse;
   float* loss_sum;
   float* logits;
-  float* part;             // [3][n_cb][Qpad]: m2, l, pick
+  float* part;             // [3][n_cb][Qpad]: m2, l, pick2
   int* counters;           // [n_rb]
   int Qpad;
-  // W mode
-  const float* lse_in;
+  float* stat;             // [2][Qpad]: row max M and lg2(sum_j 2^(s2_j - M)); written by forward, read by W mode
   Region reg[2];
   int n_regions;
 };
@@ -142,7 +148,9 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     int acc = 0;                     // mask buffer of the current tile
     int stage = 0;
     uint32_t phase = 0;
-    // forward: statistics of the row block in progress (thread = row), flushed when the row block changes
+    // forward: statistics of the row block in progress (thread = row), flushed when the row block changes.  l is the
+    // sum of 2^(s2 - m2) over the row's columns so far LESS the one term of the maximum (exactly 1): a row whose label
+    // wins by a margin keeps its tiny loss in l instead of losing it below the ulp of 1 + l.
     float m2 = -INFINITY, l = 0.f, pick = 0.f;
     int cur_rb = -1;
     auto cta_of = [&](int t) {       // inverse of the contiguous tile ranges above
@@ -175,18 +183,25 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           float M = -INFINITY;
 #pragma unroll 4
           for (int b = 0; b < nslots; ++b) M = fmaxf(M, __ldcg(base + (long long)b * p.Qpad));
-          float L = 0.f, P = 0.f;
+          float L = 0.f, P = 0.f;                              // L: the row's sum less its maximum term
+          bool top = false;                                    // the maximum term of one slot with mb == M is left out
           const float Mf = (M == -INFINITY) ? 0.f : M;       // all-masked row: every l is 0
 #pragma unroll 4
           for (int b = 0; b < nslots; ++b) {
             const float mb = __ldcg(base + (long long)b * p.Qpad);
             const float lb = __ldcg(base + plane + (long long)b * p.Qpad);
             P += __ldcg(base + 2 * plane + (long long)b * p.Qpad);   // one slot saw the label, the others hold 0
-            L = fmaf(lb, ex2_approx(mb - Mf), L);              // mb = -inf: lb = 0 and ex2(-inf) = 0
+            if (!top && mb == M) { L += lb; top = true; }
+            else { const float r = ex2_approx(mb - Mf); L += fmaf(lb, r, r); }   // mb = -inf: lb = 0, ex2(-inf) = 0
           }
-          const float lse = (M == -INFINITY) ? -INFINITY : (M + lg2_approx(L)) * LN2;
+          // loss = lse - logit[label] = (M - pick2) ln2 + ln(1 + L): exact 0 difference when the label is the maximum,
+          // and log1p keeps a fitted row's loss (L down to 1e-30) to a few ulp of itself
+          const float lnL = log1pf(L);
+          p.stat[row] = M;
+          p.stat[p.Qpad + row] = lnL * LOG2E;
+          const float lse = (M == -INFINITY) ? -INFINITY : fmaf(M, LN2, lnL);
           p.lse[row] = lse;
-          loss = lse - P;
+          loss = (M == -INFINITY) ? lse - P * LN2 : fmaf(M - P, LN2, lnL);
         }
         loss = warp_sum(loss);
         if (lane == 0 && p.loss_sum != nullptr) atomicAdd(p.loss_sum, loss);
@@ -275,17 +290,31 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           }
           if (lab >= col0 && lab < col0 + 32) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) if (lab == col0 + j) pick = s2[j] * LN2;
+            for (int j = 0; j < 32; ++j) if (lab == col0 + j) pick = s2[j];
           }
-          if (cmax > m2) { l *= ex2_approx(m2 - cmax); m2 = cmax; }   // m2 = -inf: l is 0, ex2(-inf) = 0
+          bool skip = false;                                   // a new maximum: its own term (1) stays out of l
+          if (cmax > m2) {                                     // the old maximum term joins l, rescaled
+            const float r = ex2_approx(m2 - cmax);             // m2 = -inf: l is 0, ex2(-inf) = 0
+            l = fmaf(l, r, r);
+            m2 = cmax;
+            skip = true;
+          }
           if (m2 != -INFINITY) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) l += ex2_approx(s2[j] - m2);
+            for (int j = 0; j < 32; ++j) {
+              const float e = ex2_approx(s2[j] - m2);
+              if (skip && s2[j] == m2) skip = false;           // an equal second maximum adds its 1 to l
+              else l += e;
+            }
           }
           __syncwarp();
         }
       } else {
-        const float lse2 = row_ok ? p.lse_in[row] * LOG2E : INFINITY;
+        // p = 2^((s2 - M) - lg2(1 + L)) from the forward's row statistics: s2 - M is exact near the maximum, so every p
+        // of a row carries only its own rounding and the row of W sums to 0 to a few ulp of 1 (a lse rounded at
+        // |logit| would scale the whole row by 1 + O(ulp(|logit|)))
+        const float m2r = row_ok ? p.stat[row] : INFINITY;
+        const float lgr = row_ok ? p.stat[p.Qpad + row] : 0.f;
         const int lrow = rb * TM + tid;                       // row inside the region's W array
 #pragma unroll 1
         for (int c = 0; c < 4; ++c) {
@@ -302,7 +331,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
               float v = __uint_as_float(r[j + e]) * sc2 + mk[c * 32 + j + e];
               if (p.pair_mask != nullptr && row_ok && col0 + j + e < p.C && p.pair_mask[(long long)row * p.C + col0 + j + e] != 0)
                 v = -INFINITY;
-              float pw = ex2_approx(v - lse2);               // masked / out-of-range: ex2(-inf) = 0
+              float pw = ex2_approx((v - m2r) - lgr);        // masked / out-of-range: ex2(-inf) = 0
               if (lab == col0 + j + e) pw -= 1.f;
               w[e] = pw;
             }
@@ -354,6 +383,7 @@ int make_tmap_parts(CUtensorMap* out, const void* base, long long rows, long lon
 struct ScoreWs {
   bf16 *q3, *c3;
   float* part;
+  float* stat;
   int* counters;
   bf16 *wr_hi, *wr_lo, *wc_hi, *wc_lo;
   long long ld_wr, ld_wc;
@@ -368,6 +398,7 @@ ScoreWs plan(void* base, int Q, int C, int d, int nq, int nc) {
   w.q3 = (bf16*)cv.take(2LL * Q * d * 2);
   w.c3 = (bf16*)cv.take(2LL * C * d * 2);
   w.part = (float*)cv.take(3LL * w.n_cb * w.Qpad * 4);
+  w.stat = (float*)cv.take(2LL * w.Qpad * 4);
   w.counters = (int*)cv.take((long long)w.n_rb * 4);
   w.ld_wr = (C + 7) & ~7LL; w.ld_wc = ((long long)nc + 7) & ~7LL;
   w.wr_hi = (bf16*)cv.take((long long)nq * w.ld_wr * 2);
@@ -426,6 +457,7 @@ int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
   p.Q = Q; p.C = C; p.d = d; p.k_blocks = (d + BK - 1) / BK; p.inv_t = inv_t;
   p.col_mask = col_mask; p.pair_mask = pair_mask; p.labels = labels;
   p.lse = lse; p.loss_sum = loss_sum; p.logits = logits; p.part = w.part; p.counters = w.counters; p.Qpad = w.Qpad;
+  p.stat = w.stat;
   p.n_regions = 1;
   p.reg[0] = Region{0, Q, 0, C, w.n_rb, w.n_cb, nullptr, nullptr, 0};
   const int tiles = w.n_rb * w.n_cb;
@@ -450,7 +482,8 @@ int score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const int64_
   if (int rc = make_tmap_parts(&tc, w.c3, C, d)) return rc;
   ScoreParams p = {};
   p.Q = Q; p.C = C; p.d = d; p.k_blocks = (d + BK - 1) / BK; p.inv_t = inv_t;
-  p.col_mask = col_mask; p.pair_mask = pair_mask; p.labels = labels; p.lse_in = lse;
+  p.col_mask = col_mask; p.pair_mask = pair_mask; p.labels = labels;
+  p.stat = w.stat; p.Qpad = w.Qpad;                          // the forward's row statistics (lse is not read)
   int nreg = 0;
   const bool want_dq = nq > 0 && dq != nullptr, want_dc = nc > 0 && dc != nullptr;
   if (want_dq) p.reg[nreg++] = Region{q0, nq, 0, C, (nq + TM - 1) / TM, (C + TN - 1) / TN, w.wr_hi, w.wr_lo, w.ld_wr};

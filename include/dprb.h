@@ -180,6 +180,10 @@ int dprb_attn_cls_bwd(const void* qkv_bf16, const float* probs, const void* dctx
  * fp32 accumulate): logits agree with the fp32 product of dpr_task.py:99 to a few 1e-6 of max|logit|.  Backward
  * RECOMPUTES the tiles of the rank-local row block and column block (no stored logits) and runs dq = W_rows c,
  * dc = W_cols^T q on the library's GEMM.
+ * The softmax is taken relative to each row's max: the forward leaves the row max and log-sum in the workspace and
+ * the backward builds W = softmax - onehot from them, so every row of W sums to 0 within a few ulp of 1, and the loss
+ * of a row whose label wins by a margin keeps fp32 relative accuracy, at any |logit| (raw dot products in the
+ * hundreds).  The backward's `lse` argument is not read; it is the forward's output, kept for the ABI.
  *   nq / nc: the local row / column counts backward will ask for (sizes the workspace; -1 = all).
  *   workspace: caller-owned, 256-byte aligned, >= dprb_score_tc_workspace_bytes(...); it carries the operand splits
  *   from the forward call to the backward call of the same step.
