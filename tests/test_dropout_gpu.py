@@ -10,9 +10,10 @@ pytestmark = pytest.mark.gpu
 P = 0.1
 
 
-def _masks(enc, N, S, H, heads, layers):
+def _masks(p, seed, N, S, H, heads, layers):
+    """The multipliers keep / (1 - p) of all four dropout sites of one forward's seed (`enc.last_dropout`), as the
+    oracle's `dropout=` argument takes them."""
     from dpr_scale_b200 import ops
-    p, seed = enc.last_dropout
     assert abs(p - P) < 1e-7
     sc = 1.0 / (1.0 - round(p * 65536) / 65536.0)  # the kernels quantise p to 16 bits
     T = N * S
@@ -41,7 +42,7 @@ def test_dropout_matches_oracle_with_replayed_masks():
     rep = enc(tokens)
     (rep * probe.cuda()).sum().backward()
     torch.cuda.synchronize()
-    masks = _masks(enc, N, S, 128, 2, 2)
+    masks = _masks(*enc.last_dropout, N, S, 128, 2, 2)
     keep_rate = float((masks[0]["attn"] > 0).float().mean())
     assert abs(keep_rate - (1 - P)) < 0.02, keep_rate
     sd = {k: v.clone().requires_grad_(True) for k, v in sub(g, "sd_c/").items()}

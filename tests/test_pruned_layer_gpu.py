@@ -24,7 +24,6 @@ compared block and the measured errors are printed):
 import os
 import subprocess
 import sys
-import types
 
 import numpy as np
 import pytest
@@ -419,7 +418,7 @@ def test_pruned_layer_matches_unpruned_and_float64(unpruned, H, S, p):
     enc, tokens, probe = _enc_case(H, S, p)
     masks = None
     if p:   # the masks of the run's dropout seed, replayed in the oracle
-        masks = _masks(types.SimpleNamespace(last_dropout=got["last_dropout"]), N_SEQ, S, H, H // 64, 1)
+        masks = _masks(*got["last_dropout"], N_SEQ, S, H, H // 64, 1)
         masks = {"emb": masks["emb"].double(), 0: {k: v.double() for k, v in masks[0].items()}}
     sd = {k: v.detach().double().clone().requires_grad_(True) for k, v in enc.state_dict().items()}
     ocfg = {"layers": 1, "heads": H // 64, "ln_eps": 1e-12, "pad_id": 0, "roberta": False}
