@@ -51,7 +51,7 @@ struct SearchParams {
   int d;
   int k;
   int kblocks;          // ceil(d / 64)
-  long long tiles;      // ceil(N / 256)
+  long long tiles;      // ceil(N / 128)
   long long tiles_per_part;
   u64* queues;          // [gridDim.x][gridDim.y * 128][CAP]
   int* counts;          // [gridDim.x][gridDim.y * 128]
@@ -70,6 +70,7 @@ __device__ __forceinline__ float unord_u32(uint32_t u) {
   return __uint_as_float((u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u);
 }
 __device__ __forceinline__ u64 make_key(float v, uint32_t idx) {
+  if (v == 0.0f) v = 0.0f;   // -0 and +0 are equal scores: one key, so the tie goes to the lower index
   return ((u64)ord_u32(v) << 32) | (u64)(~idx);        // larger key = better score, then lower index
 }
 __device__ __forceinline__ float key_score(u64 key) { return unord_u32((uint32_t)(key >> 32)); }

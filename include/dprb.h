@@ -400,14 +400,16 @@ int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bia
  * through wgmma and a running top-k is kept per query; no score matrix is written.
  *   queries [Q, d], corpus [N, d]: row-major 16-bit (dtype 0 = fp16 as in build_index() :178-190, 1 = bf16),
  *   d % 8 == 0, 16-byte aligned, N < 2^31 - 256, 1 <= k <= min(N, 1024).
- *   out_scores [Q, k] fp32 (fp32-accumulated inner products, descending; ties towards the lower row id),
+ *   out_scores [Q, k] fp32 (fp32-accumulated inner products, descending; equal scores, -0 and +0 included, go to
+ *   the lower row id),
  *   out_index  [Q, k] int64 = corpus row id + index_offset (the shard offset of :225-227).
  *   workspace: >= dprb_search_workspace_bytes(Q, k) bytes of device memory, caller-owned.
  *   dtype | DPRB_SEARCH_RANK_FP16: rank by (and return) the score ROUNDED TO fp16 - what the reference's topk sees,
  *   because its einsum on fp16 tensors returns fp16 (:150-151).  Ids then equal the reference's wherever its fp16
  *   scores are distinct; the default ranks by the exact fp32-accumulated score (a finer, deterministic order).
  * dprb_topk_merge replaces the per-shard merge of :272-277 (topk over the concatenated shard results + gather):
- *   scores / index [Q, total] -> the k best per row (ties towards the earlier position), workspace
+ *   scores / index [Q, total] -> the k best per row (equal scores, -0 and +0 included, go to the earlier
+ *   position), workspace
  *   >= dprb_topk_merge_workspace_bytes(Q, total).
  * ------------------------------------------------------------------------------------------- */
 enum { DPRB_SEARCH_RANK_FP16 = 0x100 };

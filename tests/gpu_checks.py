@@ -630,15 +630,29 @@ for _H in (256, 320, 768, 1024):
 
 
 # ------------------------------------------------------------------ retrieval
-def check_search(Q=100, N=5000, d=768, k=100, bf16=False, seed=20, mode="random", offset=0):
+def _r16(x):
+    """float64 -> fp16 value (as float64), rounded through fp32.  Every score the kernel rounds is an fp32 value v with
+    fl32(e - tol) <= v <= fl32(e + tol), and rounding is monotone, so bounds taken this way hold for its fp16 scores."""
+    return x.float().half().double()
+
+
+def check_search(Q=100, N=5000, d=768, k=100, bf16=False, seed=20, mode="random", offset=0, reference_ranking=False):
     """dprb_search_topk vs oracle/retrieval.py (restating run_retrieval_pytorch.py:141-176) on float64 scores.
 
+    The float64 scores of the 16-bit operands (products of 16-bit values are exact in double) are computed on the GPU,
+    a block of queries at a time, and ranked like oracle/retrieval.topk_desc (descending, ties by ascending row id).
     Tolerance: the kernel ranks by fp32-accumulated products of the identical 16-bit operands, so a returned score
-    may differ from the float64 score of the same row by tol = 1e-5 * max_row(|q|.|c|); ids must agree with the
-    oracle wherever scores are separated by more than 2 tol, and the returned set must be a valid top-k up to 2 tol.
+    may differ from the float64 score e of the same row by tol = 1e-5 * max_row(|q|.|c|).
+      * always: ids in range and distinct per query; scores non-increasing; equal scores in ascending id order.
+      * default ranking: |returned - e| <= tol; ids agree with the oracle wherever scores are separated by more than
+        2 tol, and the returned set is a valid top-k up to 2 tol.
+      * reference_ranking (the fp16-rounded score, r16): a returned score h of a row lies in
+        [r16(e - tol), r16(e + tol)].  A row is certain when r16(e - tol) == r16(e + tol): its fp16 score is known.  A certain row must be returned
+        when that score is above the k-th returned score, or equal to it with an id below the largest returned id at
+        that score.
+    Modes with a known answer are checked exactly: "constant" (identical rows), "signed_zero_f16" and "zero_query"
+    (every score is zero, -0 or +0) return rows 0..k-1 with one score.
     """
-    import numpy as np
-    from oracle import retrieval as R
     g = torch.Generator().manual_seed(seed)
     q = torch.randn(Q, d, generator=g)
     if mode == "random":
@@ -650,60 +664,112 @@ def check_search(Q=100, N=5000, d=768, k=100, bf16=False, seed=20, mode="random"
         v = torch.randn(d, generator=g)
         q = q * 0.05 + v
         c = v[None, :] * (0.25 + torch.arange(N, dtype=torch.float32)[:, None] / N)
+    elif mode == "descending":   # the best rows come first: the bar is final after the first tile
+        v = torch.randn(d, generator=g)
+        q = q * 0.05 + v
+        c = v[None, :] * (1.25 - torch.arange(N, dtype=torch.float32)[:, None] / N)
     elif mode == "constant":     # every row identical: all scores tie, the answer is rows 0..k-1 for every query
         c = torch.randn(1, d, generator=g).expand(N, d).contiguous()
+    elif mode == "negative":     # every score below 0
+        q = q.abs() + 0.1
+        c = -(torch.randn(N, d, generator=g).abs() + 0.1)
+    elif mode == "signed_zero_f16":
+        # q . c = +-2^-26 exactly in fp32; rounded to fp16 (below half the least subnormal 2^-24) every score is -0
+        # (even rows) or +0 (odd rows): all equal, so the answer is rows 0..k-1
+        assert reference_ranking, "signed_zero_f16 ranks by the fp16-rounded score"
+        q = torch.zeros(Q, d)
+        q[:, 0] = 2.0 ** -12
+        c = torch.zeros(N, d)
+        c[:, 0] = 2.0 ** -14 * (1.0 - 2.0 * (torch.arange(N) % 2 == 0).float())
+    elif mode == "zero_query":   # zero queries: every score is 0 (a sum of -0 products against the all-negative rows)
+        q = torch.zeros(Q, d)
+        c = torch.randn(N, d, generator=g)
+        c[::3] = -(c[::3].abs() + 0.1)
     else:
         raise ValueError(mode)
     dt = torch.bfloat16 if bf16 else torch.float16
-    q16, c16 = q.to(dt), c.to(dt)
-    s, i = ops.search_topk(q16.to(DEV), c16.to(DEV), k, index_offset=offset)
+    q16, c16 = q.to(dt).to(DEV), c.to(dt).to(DEV)
+    s, i = ops.search_topk(q16, c16, k, index_offset=offset, reference_ranking=reference_ranking)
     torch.cuda.synchronize()
-    s, i = s.cpu().numpy().astype(np.float64), i.cpu().numpy() - offset
-    qe, ce = q16.double().numpy(), c16.double().numpy()
-    exact = qe @ ce.T
-    tol = 1e-5 * float((np.abs(qe) @ np.abs(ce).T).max())
-    out = {"tol": tol}
     assert s.shape == (Q, k) and i.shape == (Q, k)
-    assert (i >= 0).all() and (i < N).all(), "row ids out of range"
-    assert all(len(set(r)) == k for r in i), "duplicate row ids"
-    ds = np.diff(s, axis=1)
-    assert (ds <= 0).all(), "scores not descending"
-    assert (np.diff(i, axis=1)[ds == 0] > 0).all(), "equal scores not ordered by ascending row id"
-    got = np.take_along_axis(exact, i, axis=1)
-    out["score_maxerr"] = float(np.abs(got - s).max())
-    assert out["score_maxerr"] <= tol, f"score error {out['score_maxerr']:.3e} > {tol:.3e}"
-    os_, oi = R.topk_desc(exact, min(k + 1, N))
-    kth = os_[:, k - 1]
-    assert (got >= kth[:, None] - 2 * tol).all(), "returned a row that is not in the top-k"
-    mism = 0
-    for r in range(Q):
-        must = oi[r, :k][os_[r, :k] > kth[r] + 2 * tol]
-        assert set(must) <= set(i[r]), f"query {r}: missing rows with score above the k-th"
-        e = os_[r]
-        for j in range(k):
-            lo = e[j] - e[j + 1] if j + 1 < len(e) else np.inf
-            hi = e[j - 1] - e[j] if j > 0 else np.inf
-            if lo > 2 * tol and hi > 2 * tol:
-                assert i[r, j] == oi[r, j], f"query {r} rank {j}: {i[r, j]} vs oracle {oi[r, j]}"
-            else:
-                mism += int(i[r, j] != oi[r, j])
-    out["near_tie_swaps"] = mism
+    s, i = s.double(), i - offset
+    assert bool(((i >= 0) & (i < N)).all()), "row ids out of range"
+    assert bool((i.sort(1).values.diff(1) != 0).all()), "duplicate row ids"
+    ds = s.diff(1)
+    assert bool((ds <= 0).all()), "scores not descending"
+    assert bool((i.diff(1)[ds == 0] > 0).all()), "equal scores not ordered by ascending row id"
+    if mode in ("constant", "signed_zero_f16", "zero_query"):
+        assert torch.equal(i, torch.arange(k, device=DEV).expand(Q, k)), "tied rows not returned as 0..k-1"
+        assert bool((s == s[:, :1]).all()), "tied rows returned with different scores"
+        if mode != "constant":
+            assert bool((s == 0).all()), "zero scores returned as nonzero"
+
+    qe, ce = q16.double(), c16.double()
+    QC = max(1, (1 << 25) // N)          # float64 score blocks of <= 256 MB
+    tol = 1e-5 * max(float((qe[a:a + QC].abs() @ ce.abs().T).max()) for a in range(0, Q, QC))
+    out = {"tol": tol}
+    maxerr = 0.0
+    mism = certain = 0
+    rows = torch.arange(N, device=DEV)
+    for a in range(0, Q, QC):
+        exact = qe[a:a + QC] @ ce.T
+        sb, ib = s[a:a + QC], i[a:a + QC]
+        got = exact.gather(1, ib)
+        returned = torch.zeros_like(exact, dtype=torch.bool).scatter_(1, ib, True)
+        if reference_ranking:
+            assert bool(((_r16(got - tol) <= sb) & (sb <= _r16(got + tol))).all()), \
+                "fp16 score outside [r16(e - tol), r16(e + tol)]"
+            lo16 = _r16(exact - tol)
+            sure = lo16 == _r16(exact + tol)
+            hk = sb[:, -1:]
+            last = torch.where(sb == hk, ib, -1).max(1, keepdim=True).values
+            must = sure & ((lo16 > hk) | ((lo16 == hk) & (rows[None, :] < last)))
+            assert bool(returned[must].all()), "missing a row whose fp16 score is certain to rank in the top-k"
+            certain += int(sure.sum())
+            continue
+        maxerr = max(maxerr, float((got - sb).abs().max()))
+        assert maxerr <= tol, f"score error {maxerr:.3e} > {tol:.3e}"
+        os_, oi = exact.sort(dim=1, descending=True, stable=True)
+        os_, oi = os_[:, :k + 1], oi[:, :k + 1]
+        kth = os_[:, k - 1:k]
+        assert bool((got >= kth - 2 * tol).all()), "returned a row that is not in the top-k"
+        must = os_[:, :k] > kth + 2 * tol
+        assert bool(returned.gather(1, oi[:, :k])[must].all()), "missing rows with score above the k-th"
+        inf = torch.full_like(kth, math.inf)
+        gap = os_[:, :-1] - os_[:, 1:]                        # gap[:, j] = e[j] - e[j + 1]
+        lo = torch.cat([gap, inf], 1)[:, :k]
+        hi = torch.cat([inf, gap], 1)[:, :k]
+        sep = (lo > 2 * tol) & (hi > 2 * tol)
+        same = ib == oi[:, :k]
+        assert bool(same[sep].all()), "ids differ from the oracle where scores are separated by more than 2 tol"
+        mism += int((~same & ~sep).sum())
+    if reference_ranking:
+        out["certain_rows"] = certain
+    else:
+        out["score_maxerr"] = maxerr
+        out["near_tie_swaps"] = mism
     return out
 
 
-def check_topk_merge(Q=37, total=300, k=100, seed=30):
+def check_topk_merge(Q=37, total=300, k=100, seed=30, signed_zero=False):
     """dprb_topk_merge vs the restated shard merge (run_retrieval_pytorch.py:272-277: topk over the concatenated shard
-    results + gather); bit-exact (fp32 compare / select only), ties towards the earlier position."""
+    results + gather); bit-exact (fp32 compare / select only), ties towards the earlier position.
+    signed_zero: -0.0 at even and +0.0 at odd positions, all equal scores, so the answer is positions 0..k-1."""
     import numpy as np
     from oracle import retrieval as R
     g = torch.Generator().manual_seed(seed)
     s = torch.randn(Q, total, generator=g)
     nt = min(s[:, ::7].shape[1], s[:, 3::7].shape[1])
     s[:, 0:7 * nt:7] = s[:, 3:3 + 7 * nt:7]                  # inject exact ties
+    if signed_zero:
+        s = torch.zeros(Q, total)
+        s[:, 0::2] = -0.0
     idx = torch.randint(0, 2 ** 40, (Q, total), generator=g, dtype=torch.int64)
     ms, mi = ops.topk_merge(s.to(DEV), idx.to(DEV), k)
     torch.cuda.synchronize()
     rs, order = R.topk_desc(s.numpy().astype(np.float64), k)
+    if signed_zero:
+        assert np.array_equal(order, np.broadcast_to(np.arange(k), (Q, k)))
     ri = np.take_along_axis(idx.numpy(), order, axis=1)
     assert np.array_equal(ms.cpu().numpy().astype(np.float64), rs), "merged scores differ"
     assert np.array_equal(mi.cpu().numpy(), ri), "merged ids differ"
