@@ -104,6 +104,10 @@ SIGNATURES = {
     "dprb_expert_search_workspace_bytes": (c_int64, [c_int64, c_int]),
     "dprb_expert_search": (c_int, [_P, _P, _P, c_int64, c_int, c_int, c_int, _P, c_int, c_int, _P, c_int64, _P, _P,
                                    c_int64, _P, c_int, _P, _P, c_int, c_int, c_int, _P, _P, _P, c_int64, _P]),
+    "dprb_sparse_search_block_queries": (c_int, [c_int64]),
+    "dprb_sparse_search_workspace_bytes": (c_int64, [c_int64, c_int]),
+    "dprb_sparse_search": (c_int, [_P, _P, _P, c_int64, c_int, _P, c_int64, _P, _P, _P, _P, c_int, c_int, c_int, c_int,
+                                   _P, _P, _P, c_int64, _P]),
     "dprb_sqerr_workspace_bytes": (c_int64, [c_int, c_int]),
     "dprb_sqerr_fwd": (c_int, [_P, c_int64, _P, c_int64, c_int, c_int, _P, _P, c_int64, _P, c_int64, _P]),
 }

@@ -216,6 +216,18 @@ int dprb_expert_search(const void* payload, const int32_t* row, const int32_t* t
                        reinterpret_cast<long long*>(out_ids), workspace, workspace_bytes, S(stream));
 }
 
+int dprb_sparse_search_block_queries(int64_t N) { return sparse_search_block_queries(N); }
+int64_t dprb_sparse_search_workspace_bytes(int64_t N, int Qb) { return sparse_search_workspace_bytes(N, Qb); }
+int dprb_sparse_search(const int32_t* row, const void* weight, const int64_t* term_ptr, int64_t nnz, int V,
+                       const int64_t* row_ids, int64_t N, const int32_t* q_term, const float* q_weight,
+                       const int32_t* q_seq, const int32_t* item_end, int Eq, int items, int Qb, int k,
+                       float* out_scores, int64_t* out_ids, void* workspace, int64_t workspace_bytes,
+                       dprb_stream_t stream) {
+  return sparse_search(row, weight, reinterpret_cast<const long long*>(term_ptr), nnz, V,
+                       reinterpret_cast<const long long*>(row_ids), N, q_term, q_weight, q_seq, item_end, Eq, items,
+                       Qb, k, out_scores, reinterpret_cast<long long*>(out_ids), workspace, workspace_bytes, S(stream));
+}
+
 int64_t dprb_sqerr_workspace_bytes(int rows, int d) {
   (void)d;
   return sqerr_workspace_bytes(rows);

@@ -127,12 +127,32 @@ int expert_group(const int32_t* ids, const float* w, const int32_t* mask, const 
                  int32_t* out_expert, int32_t* out_seq, int32_t* out_tok, float* out_w, float* out_payload,
                  void* workspace, long long workspace_bytes, cudaStream_t stream);
 
+// fixed_select.cu: the int64 fixed-point accumulator [Qb, N] at 2^-32 of the index searches, and its per-query top-k.
+// fixed_acc_init carves the accumulator and a work counter from the workspace and zeroes both on the stream;
+// fixed_acc_select writes the k best rows of every query (descending, ties towards the lower row), as row_ids[row].
+struct FixedAcc {
+  unsigned long long* acc;
+  int* counter;
+};
+int fixed_acc_block_queries(long long N);
+long long fixed_acc_workspace_bytes(long long N, int Qb);
+int fixed_acc_init(void* workspace, long long N, int Qb, FixedAcc* out, cudaStream_t stream);
+int fixed_acc_select(const unsigned long long* acc, long long N, int Qb, int k, const long long* row_ids,
+                     float* out_scores, long long* out_ids, cudaStream_t stream);
+
 int expert_search_block_queries(long long N);
 long long expert_search_workspace_bytes(long long N, int Qb);
 int expert_search(const void* payload, const int32_t* row, const int32_t* tile_bounds, long long E, int T, int P,
                   int ldp, const void* cls, int Pc, int ldc, const long long* row_ids, long long N,
                   const void* q_payload, const int32_t* q_seq, long long Eq, const void* q_cls, int Qb,
                   const int32_t* groups, const int32_t* item_end, int G, int items, int k, float* out_scores,
+                  long long* out_ids, void* workspace, long long workspace_bytes, cudaStream_t stream);
+
+int sparse_search_block_queries(long long N);
+long long sparse_search_workspace_bytes(long long N, int Qb);
+int sparse_search(const int32_t* row, const void* weight, const long long* term_ptr, long long nnz, int V,
+                  const long long* row_ids, long long N, const int32_t* q_term, const float* q_weight,
+                  const int32_t* q_seq, const int32_t* item_end, int Eq, int items, int Qb, int k, float* out_scores,
                   long long* out_ids, void* workspace, long long workspace_bytes, cudaStream_t stream);
 
 long long sqerr_workspace_bytes(int rows);

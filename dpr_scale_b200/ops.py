@@ -736,3 +736,68 @@ def expert_search(payload, row, tile_bounds, P, cls, row_ids, q_payload, q_seq, 
                                  groups.shape[0], int(items), int(k), _ptr(scores), _ptr(ids), buf.data_ptr() + off,
                                  buf.numel() - off, _stream()), "dprb_expert_search")
     return scores, ids
+
+
+SPARSE_SEARCH_TILE = 2048         # include/dprb.h DPRB_SPARSE_SEARCH_TILE: postings per work item
+SPARSE_SEARCH_MAX_K = 1024
+
+
+def sparse_search_check(V, nnz, N, k):
+    """ValueError for the shapes dprb_sparse_search refuses (host-only: needs no GPU)."""
+    if not 1 <= V < 1 << 31:
+        raise ValueError(f"sparse search needs a vocabulary of 1 .. 2^31 - 1 terms (got {V})")
+    if not 0 <= nnz < 1 << 40:
+        raise ValueError(f"sparse search needs fewer than 2^40 postings (got {nnz})")
+    if not 1 <= N < 1 << 31:
+        raise ValueError(f"sparse search needs 1 .. 2^31 - 1 passages (got {N})")
+    if not 1 <= k <= min(SPARSE_SEARCH_MAX_K, N):
+        raise ValueError(f"sparse search needs 1 <= topk <= min({SPARSE_SEARCH_MAX_K}, passages={N}) (got {k})")
+
+
+def sparse_search_block_queries(N):
+    """Queries per search block: the [Qb, N] int64 accumulator stays within the library's fixed 2 GiB budget."""
+    return int(_lib.load().dprb_sparse_search_block_queries(int(N)))
+
+
+def sparse_search_items(term_ptr, q_term):
+    """Work items of one query block: term_ptr host int64 [V + 1], q_term host int [Eq] -> (item_end int32 [Eq], items),
+    each entry owning ceil(postings of its term / SPARSE_SEARCH_TILE) items."""
+    q_term = np.asarray(q_term, dtype=np.int64)
+    n = term_ptr[q_term + 1] - term_ptr[q_term]
+    end = np.cumsum((n + SPARSE_SEARCH_TILE - 1) // SPARSE_SEARCH_TILE)
+    items = int(end[-1]) if end.size else 0
+    if items >= 1 << 31:
+        raise ValueError(f"sparse search block has {items} work items (2^31 or more): search fewer queries at once")
+    return end.astype(np.int32), items
+
+
+_SPARSE_SEARCH_WS = {}
+
+
+def sparse_search(row, weight, term_ptr, nnz, row_ids, q_term, q_weight, q_seq, Qb, item_end, items, k):
+    """One query block through dprb_sparse_search (include/dprb.h).  Index: row int32 / weight fp16 [>= nnz rounded up
+    to 8], term_ptr int64 [V + 1], row_ids int64 [N] (the id returned for each row).  Queries: q_term int32 [Eq] in
+    [0, V), q_weight fp32 [Eq], q_seq int32 [Eq] in [0, Qb), item_end int32 [Eq] / items from sparse_search_items
+    (all device tensors).  Returns (scores fp32 [Qb, k], ids int64 [Qb, k])."""
+    lib = _lib.load()
+    dev = row_ids.device
+    N, V, Eq = row_ids.numel(), term_ptr.numel() - 1, q_term.numel()
+    assert row.dtype == torch.int32 and weight.dtype == torch.float16 and term_ptr.dtype == torch.int64
+    assert row.numel() >= (nnz + 7) // 8 * 8 and weight.numel() >= (nnz + 7) // 8 * 8
+    assert q_term.dtype == torch.int32 and q_weight.dtype == torch.float32 and q_seq.dtype == torch.int32
+    assert item_end.dtype == torch.int32 and item_end.numel() == Eq and q_weight.numel() == Eq == q_seq.numel()
+    for t in (row, weight, term_ptr, row_ids, q_term, q_weight, q_seq, item_end):
+        assert t.is_contiguous() and t.device == dev
+    nbytes = int(lib.dprb_sparse_search_workspace_bytes(N, int(Qb)))
+    buf = _SPARSE_SEARCH_WS.get(dev)
+    if buf is None or buf.numel() < nbytes + 256:
+        _SPARSE_SEARCH_WS[dev] = None                          # free the old buffer before taking the new one
+        buf = _SPARSE_SEARCH_WS[dev] = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+    off = (-buf.data_ptr()) % 256
+    scores = torch.empty(Qb, k, dtype=torch.float32, device=dev)
+    ids = torch.empty(Qb, k, dtype=torch.int64, device=dev)
+    check(lib.dprb_sparse_search(_ptr(row), _ptr(weight), _ptr(term_ptr), int(nnz), int(V), _ptr(row_ids), N,
+                                 _ptr(q_term), _ptr(q_weight), _ptr(q_seq), _ptr(item_end), int(Eq), int(items),
+                                 int(Qb), int(k), _ptr(scores), _ptr(ids), buf.data_ptr() + off, buf.numel() - off,
+                                 _stream()), "dprb_sparse_search")
+    return scores, ids

@@ -452,6 +452,34 @@ int dprb_expert_search(const void* payload, const int32_t* row, const int32_t* t
                        int64_t* out_ids, void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Retrieval from a sparse vocabulary index (SPLADE first-stage retrieval).  For every query q of a block of Qb queries
+ * and every passage row d in [0, N):
+ *   score(q, d) = sum over q's entries (t, w_q) of sum over d's postings (t, w_p) of w_q * w_p
+ * and the k best rows per query, descending, ties towards the lower row; out_ids [Qb, k] int64 = row_ids[row] (or the
+ * row when row_ids is NULL), out_scores [Qb, k] fp32.
+ * Index: postings sorted by term and, within a term, by row: row int32 [nnz] in [0, N), weight fp16 [nnz]; both
+ *   16-byte aligned and allocated for nnz rounded up to a multiple of 8 entries (the padding is read, never used);
+ *   term_ptr int64 [V + 1]: term t's postings are [term_ptr[t], term_ptr[t + 1]).
+ * Queries: q_term int32 [Eq] in [0, V), q_weight fp32 [Eq], q_seq int32 [Eq] in [0, Qb) (entries in any order; a
+ *   term may repeat).  Each entry's postings are cut into ceil(len / DPRB_SPARSE_SEARCH_TILE) tiles; item_end int32
+ *   [Eq]: inclusive prefix sums of the entries' tile counts; items = item_end[Eq - 1].
+ * Every product w_q * w_p is formed in fp32 and added as int64 fixed point at 2^-32 (the caller keeps each query's sum
+ * of |products| below 2^30), so the result is bitwise repeatable and a query's result does not depend on its block.
+ * Requires 1 <= N < 2^31, V >= 1, 0 <= nnz < 2^40, Eq >= 0, 1 <= k <= min(1024, N),
+ * 1 <= Qb <= dprb_sparse_search_block_queries(N) (a fixed accumulator budget of 2 GiB); checked before any launch
+ * (return code 1).  workspace: >= dprb_sparse_search_workspace_bytes(N, Qb) bytes, 256-byte aligned.  Enqueues two
+ * memsets and two launches; never synchronises.
+ * ------------------------------------------------------------------------------------------- */
+enum { DPRB_SPARSE_SEARCH_TILE = 2048 };
+int dprb_sparse_search_block_queries(int64_t N);
+int64_t dprb_sparse_search_workspace_bytes(int64_t N, int Qb);
+int dprb_sparse_search(const int32_t* row, const void* weight, const int64_t* term_ptr, int64_t nnz, int V,
+                       const int64_t* row_ids, int64_t N, const int32_t* q_term, const float* q_weight,
+                       const int32_t* q_seq, const int32_t* item_end, int Eq, int items, int Qb, int k,
+                       float* out_scores, int64_t* out_ids, void* workspace, int64_t workspace_bytes,
+                       dprb_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Squared-error sum for query-encoder distillation (MSELoss(reduction="sum") of the reference's DPRDistillTask,
  * dpr_scale/task/dpr_distill_task.py:43, :167, :186, and the gradient autograd takes through it):
  *   loss_sum[0] = sum_{r < rows, c < d} (x[r, c] - t[r, c])^2
