@@ -96,6 +96,9 @@ SIGNATURES = {
     "dprb_expert_group": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P,
                                   _P, _P, _P, _P, _P, c_int64, _P]),
     "dprb_seqcls_head_fwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
+    "dprb_seqcls_group_ce_workspace_bytes": (c_int64, [c_int, c_int]),
+    "dprb_seqcls_group_ce": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint64, _P, _P, _P, _P, _P, _P,
+                                     c_int64, _P]),
     "dprb_search_workspace_bytes": (c_int64, [c_int64, c_int]),
     "dprb_search_topk": (c_int, [_P, _P, c_int, c_int64, c_int64, c_int, c_int, c_int64, _P, _P, _P, c_int64, _P]),
     "dprb_topk_merge_workspace_bytes": (c_int64, [c_int64, c_int]),

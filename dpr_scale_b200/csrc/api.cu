@@ -190,6 +190,13 @@ int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bia
                          int H, int L, dprb_stream_t stream) {
   return seqcls_head_fwd(pre, weight, bias, logits, score, N, H, L, S(stream));
 }
+int64_t dprb_seqcls_group_ce_workspace_bytes(int B, int H) { return seqcls_group_ce_workspace_bytes(B, H); }
+int dprb_seqcls_group_ce(const float* pre, const float* weight, const float* bias, const int64_t* labels, int B, int G,
+                         int H, float dropout_p, uint64_t dropout_seed, float* loss, float* logits, void* dpre_bf16,
+                         float* dweight, float* dbias, void* workspace, int64_t workspace_bytes, dprb_stream_t stream) {
+  return seqcls_group_ce(pre, weight, bias, reinterpret_cast<const long long*>(labels), B, G, H, dropout_p,
+                         dropout_seed, loss, logits, dpre_bf16, dweight, dbias, workspace, workspace_bytes, S(stream));
+}
 int64_t dprb_search_workspace_bytes(int64_t Q, int k) { return search_workspace_bytes(Q, k); }
 int dprb_search_topk(const void* queries, const void* corpus, int dtype, int64_t Q, int64_t N, int d, int k,
                      int64_t index_offset, float* out_scores, int64_t* out_index, void* workspace,

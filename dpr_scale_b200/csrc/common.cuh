@@ -230,7 +230,10 @@ inline Drop drop_from_site(float p, uint64_t site_seed) {
   d.row_mul = (uint32_t)(site_seed >> 32) ? (uint32_t)(site_seed >> 32) : 1u;
   return d;
 }
-enum { DROP_SITE_EMBED = 0, DROP_SITE_ATTN = 1, DROP_SITE_ATTN_OUT = 2, DROP_SITE_FFN_OUT = 3 };
+enum { DROP_SITE_EMBED = 0, DROP_SITE_ATTN = 1, DROP_SITE_ATTN_OUT = 2, DROP_SITE_FFN_OUT = 3,
+       // cross-encoder classification head, layer 0: after tanh (dprb_seqcls_group_ce) and, for RoBERTa, on the CLS
+       // rows before the head's dense layer (applied by the caller from dprb_dropout_mask)
+       DROP_SITE_HEAD = 4, DROP_SITE_HEAD_IN = 5 };
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

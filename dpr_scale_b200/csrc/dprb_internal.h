@@ -105,6 +105,10 @@ int topk_merge(const float* scores, const long long* index, long long Q, int tot
 
 int seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
                     int H, int L, cudaStream_t stream);
+long long seqcls_group_ce_workspace_bytes(int B, int H);
+int seqcls_group_ce(const float* pre, const float* weight, const float* bias, const long long* labels, int B, int G,
+                    int H, float dropout_p, unsigned long long dropout_seed, float* loss, float* logits, void* dpre,
+                    float* dweight, float* dbias, void* workspace, long long workspace_bytes, cudaStream_t stream);
 
 long long encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S, int save);
 int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, cudaStream_t stream);

@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from ..transforms.dpr_distill_transform import DPRDistillTransform
-from ..transforms.dpr_transform import DPRTransform, maybe_add_title
+from ..transforms.dpr_transform import DPRCrossAttentionTransform, DPRTransform, maybe_add_title
 from ..transforms.hf_transform import HFTransform
 from ..utils.lightning_shim import LightningDataModule
 
@@ -352,8 +352,9 @@ class DenseRetrieverDataModuleBase(LightningDataModule):
 
 class DenseRetrieverJsonlDataModule(DenseRetrieverDataModuleBase):
     """DPR-format JSONL (datamodule/dpr.py:263-331); same keyword arguments, plus ``prefetch_batches`` (0 = synchronous)
-    
-    ``device_prefetch`` (stage batches on the GPU from the background thread) and ``fast_tokenize``."""
+    ``device_prefetch`` (stage batches on the GPU from the background thread) and ``fast_tokenize``.  With
+    ``use_cross_attention`` the batches are cross-encoder training groups (transforms.dpr_transform
+    DPRCrossAttentionTransform), assembled on the same background thread."""
 
     def __init__(self, transform, train_path: str, val_path: str, test_path: str, batch_size: int = 2,
                  val_batch_size: int = 0, test_batch_size: int = 0, num_positive: int = 1, num_negative: int = 7,
@@ -363,12 +364,11 @@ class DenseRetrieverJsonlDataModule(DenseRetrieverDataModuleBase):
                  prefetch_batches: int = 4, device_prefetch: bool = True, fast_tokenize: bool = True, *args,
                  **kwargs):
         super().__init__(transform)
-        if use_cross_attention:
-            raise NotImplementedError("cross-attention transform is outside the bi-encoder path (only the bi-encoder step is implemented)")
         self.batch_size = batch_size
         self.val_batch_size = val_batch_size if val_batch_size else batch_size
         self.test_batch_size = test_batch_size if test_batch_size else self.val_batch_size
-        self.dpr_transform = DPRTransform(transform, num_positive, num_negative, neg_ctx_sample, pos_ctx_sample,
+        transform_class = DPRCrossAttentionTransform if use_cross_attention else DPRTransform
+        self.dpr_transform = transform_class(transform, num_positive, num_negative, neg_ctx_sample, pos_ctx_sample,
                                           num_val_negative, num_test_negative, use_title, sep_token, rel_sample,
                                           **kwargs)
         self.num_workers = num_workers     # accepted; assembly runs on the BatchStream thread

@@ -335,6 +335,51 @@ def seqcls_head_fwd(pre, weight, bias=None):
     return logits, score
 
 
+SEQCLS_GROUP_MAX = 64    # include/dprb.h DPRB_SEQCLS_GROUP_MAX
+DROP_SITE_HEAD, DROP_SITE_HEAD_IN = 4, 5   # dropout sites (layer 0) of the cross-encoder head (include/dprb.h)
+_GROUP_CE_WS = {}
+
+
+def seqcls_group_ce_check(rows, H, G):
+    """The limits of dprb_seqcls_group_ce on the host (ValueError, no device needed); returns the number of groups."""
+    if not 2 <= G <= SEQCLS_GROUP_MAX:
+        raise ValueError(f"grouped cross-entropy needs 2 <= group size <= {SEQCLS_GROUP_MAX} (got {G})")
+    if rows <= 0 or rows % G:
+        raise ValueError(f"{rows} rows do not form whole groups of {G}")
+    if H % 8 or not 0 < H <= 1024:
+        raise ValueError(f"grouped cross-entropy needs a hidden size that is a multiple of 8 and <= 1024 (got {H})")
+    return rows // G
+
+
+def seqcls_group_ce(pre, weight, bias, labels, G, dropout_p=0.0, dropout_seed=0):
+    """Grouped softmax cross-entropy of a one-label head and its backward (include/dprb.h dprb_seqcls_group_ce):
+    pre fp32 [B*G, H], weight fp32 [1, H], bias fp32 [1] or None, labels int64 [B].  Returns (loss fp32 [1] = mean over
+    groups, logits fp32 [B*G], dpre bf16 [B*G, H], dweight fp32 [1, H], dbias fp32 [1]), the gradients of that loss."""
+    N, H = pre.shape
+    B = seqcls_group_ce_check(N, H, G)
+    if weight.shape != (1, H):
+        raise ValueError(f"grouped cross-entropy trains one label: weight must be [1, {H}] (got {tuple(weight.shape)})")
+    if labels.shape != (B,):
+        raise ValueError(f"labels must be [{B}] (got {tuple(labels.shape)})")
+    dev = pre.device
+    lib = _lib.load()
+    loss = torch.empty(1, dtype=torch.float32, device=dev)
+    logits = torch.empty(N, dtype=torch.float32, device=dev)
+    dpre = torch.empty(N, H, dtype=torch.bfloat16, device=dev)
+    dweight = torch.empty(1, H, dtype=torch.float32, device=dev)
+    dbias = torch.empty(1, dtype=torch.float32, device=dev)
+    nbytes = int(lib.dprb_seqcls_group_ce_workspace_bytes(B, H))
+    buf = _GROUP_CE_WS.get(dev)
+    if buf is None or buf.numel() < nbytes:
+        buf = _GROUP_CE_WS[dev] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    labels = labels.to(dev, torch.int64).contiguous()
+    check(lib.dprb_seqcls_group_ce(_ptr(pre.contiguous()), _ptr(weight.contiguous()), _ptr(bias), _ptr(labels), B, G, H,
+                                   float(dropout_p), int(dropout_seed) & 0xFFFFFFFFFFFFFFFF, _ptr(loss), _ptr(logits),
+                                   _ptr(dpre), _ptr(dweight), _ptr(dbias), buf.data_ptr(), buf.numel(), _stream()),
+          "dprb_seqcls_group_ce")
+    return loss, logits, dpre, dweight, dbias
+
+
 _SEARCH_WS = {}
 
 

@@ -137,3 +137,82 @@ class DPRTransform(nn.Module):
             "scores": torch.tensor(scores, dtype=torch.float32),
             "ctx_mask": torch.tensor(ctx_mask, dtype=torch.bool),
         }
+
+
+class DPRCrossAttentionTransform(DPRTransform):
+    """Cross-encoder training groups - the sampling of the reference's ``DPRCrossAttentionTransform``
+    (/root/reference/dpr_scale/transforms/dpr_transform.py:190-326): per question, its positive and then its hard
+    negatives (sampled in the train stage, truncated otherwise), and, when a row has fewer negatives than wanted, a fill
+    drawn without replacement from every positive and hard negative of the batch (``num_random_negs`` more in the train
+    stage).  The pair at position 0 of each group is the relevant one.  ``np.random`` is drawn with the reference's
+    arguments in the reference's order.
+
+    Where this departs from the reference:
+      * each (question, passage) goes through ``text_transform(questions, passages)``, the pair encoding the rerank
+        datamodule uses, so the model trains on exactly what it reranks.  The reference hands its tokenizer a
+        ``{"text", "label"}`` dict of ``" ".join([question, sep_token, passage])`` strings, which neither of its
+        transforms accepts;
+      * with ``pos_ctx_sample`` the sampled positives form the group; the reference draws them and then keeps every
+        positive, which gives groups of unequal size;
+      * rows in the DPR retriever-output format (``ctxs`` + ``has_answer``) are normalised before the batch fill is
+        collected, and a passage given as a token list is joined wherever it is used; the reference reads
+        ``positive_ctxs`` of every row first and joins the token lists of a row's own positives only, so it fails on
+        both.
+
+    The batch is ``{"text_ids": tokens [B*G, S], "labels": int64 [B] (zeros), "group_size": G}``."""
+
+    def __init__(self, text_transform, num_positive: int = 1, num_negative: int = 7, neg_ctx_sample: bool = True,
+                 pos_ctx_sample: bool = False, num_val_negative: int = 7, num_test_negative=None,
+                 use_title: bool = False, sep_token: str = " ", rel_sample: bool = False, corpus=None,
+                 text_column: str = "text", num_random_negs: int = 0):
+        super().__init__(text_transform, num_positive, num_negative, neg_ctx_sample, pos_ctx_sample, num_val_negative,
+                         num_test_negative, use_title, sep_token, rel_sample, corpus, text_column)
+        self.num_random_negs = num_random_negs
+
+    def _text(self, ctx):
+        if self.corpus is not None:
+            return self.corpus[int(ctx["docidx"])].decode("UTF-8").strip().split("\t")[1]
+        text = ctx["text"]
+        return text if isinstance(text, str) else " ".join(text)     # text given as a token list
+
+    def select(self, rows, stage="train"):
+        """The sampling half of forward(): (questions, passages), one entry per pair, group by group."""
+        rows = [_normalise_row(json.loads(raw)) for raw in rows]
+        candidates = [c for row in rows for c in row["positive_ctxs"] + row["hard_negative_ctxs"]]
+        want = self._negatives_wanted(stage)
+        extra = self.num_random_negs if stage == "train" else 0
+        questions, passages = [], []
+        for row in rows:
+            pos = row["positive_ctxs"]
+            if stage == "train" and self.pos_ctx_sample:
+                pos = _draw(pos, self.num_positive, self.rel_sample)
+            else:
+                pos = pos[: self.num_positive]
+            neg = row["hard_negative_ctxs"]
+            if want > 0:
+                if stage == "train" and self.neg_ctx_sample and len(neg) > want:
+                    neg = _draw(neg, want, self.rel_sample)
+                else:
+                    neg = neg[:want]
+            else:
+                neg = []
+            ctxs = pos + neg
+            if len(neg) < want + extra:
+                picked = np.random.choice(len(candidates), want + extra - len(neg), replace=False)
+                ctxs += [candidates[int(j)] for j in picked]
+            questions += [row["question"]] * len(ctxs)
+            passages += [self._text(c) for c in ctxs]
+        return questions, passages, len(rows)
+
+    def finish(self, selection, fast=True):
+        """The tokenisation half of forward(): one pair encoding of every (question, passage)."""
+        questions, passages, B = selection
+        if B == 0 or len(passages) % B:
+            raise ValueError(f"{len(passages)} pairs do not form {B} equal groups")
+        return {"text_ids": self.text_transform(questions, passages),
+                "labels": torch.zeros(B, dtype=torch.long),
+                "group_size": len(passages) // B}
+
+    def forward(self, batch, stage="train"):
+        rows = batch if type(batch) is list else batch[self.text_column]
+        return self.finish(self.select(rows, stage))

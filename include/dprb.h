@@ -118,7 +118,8 @@ int dprb_ln_bwd(const void* dy_bf16, const float* dy_cls, int cls_stride, const 
                 float* dbias, int T, int H, void* dzm_bf16, float dropout_p, uint64_t dropout_site_seed,
                 int z_f16, dprb_stream_t stream);
 /* Dropout sites: 0 embeddings [T,H], 1 attention probabilities [nseq*heads*S, S], 2 attention-output dense [T,H],
- * 3 FFN-output dense [T,H].  Element (r, c) of a site is kept iff its 16-bit lane of h(r, c/8, (c/2)%4, site seed)
+ * 3 FFN-output dense [T,H]; with layer 0, the cross-encoder head's 4 after tanh [N,H] (dprb_seqcls_group_ce) and 5 on
+ * RoBERTa's CLS rows before the head's dense layer [N,H].  Element (r, c) of a site is kept iff its 16-bit lane of h(r, c/8, (c/2)%4, site seed)
  * is >= round(p * 65536) - one hash chain per group of 8 columns, one multiply-xorshift finaliser per column pair
  * (csrc/common.cuh: Drop); site seed = fold32(dropout_seed + (layer*8 + site + 1) * 0x9E3779B97F4A7C15).
  * dprb_ln_bwd: dbias accumulates the column sums of the Linear's own output gradient (dzm when dropout is on).
@@ -392,6 +393,27 @@ int dprb_expert_group(const int32_t* ids, const float* w, const int32_t* mask, c
 #define DPRB_SEQCLS_MAX_LABELS 16
 int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
                          int H, int L, dprb_stream_t stream);
+/* Training the same head with one relevance label: the grouped softmax cross-entropy of a reranker trained on (question,
+ * passage) groups - candidate 0 .. G-1 of group g are rows g*G .. g*G + G-1, and labels[g] names the relevant one.  With
+ * t = tanh(pre), mask the dropout multiplier (keep / (1 - p), or 0) of site 4, layer 0 under dropout_seed - element
+ * (n, h) of dprb_dropout_mask(keep, B*G, H, p, dropout_seed, 0, 4) - and q_g = softmax over the group's logits:
+ *   logits[n]    = weight . (t[n] * mask[n]) + bias[0]           (BertForSequenceClassification's dropout + classifier,
+ *                                                                 RobertaClassificationHead's dropout + out_proj)
+ *   loss[0]      = mean over groups of (logsumexp_g - logits[g*G + labels[g]])
+ *   dlogit[n]    = (q_g[n] - [n is the label row]) / B
+ *   dpre[n, h]   = bf16(dlogit[n] * weight[h] * mask[n, h] * (1 - t[n, h]^2))      (bf16 [B*G, H], for the GEMMs)
+ *   dweight[h]   = sum_n dlogit[n] * t[n, h] * mask[n, h],   dbias[0] = sum_n dlogit[n]
+ * The caller back-propagates dpre through the dense layer with dprb_gemm_bf16 / dprb_colsum_bf16.  dweight, dbias and
+ * loss are summed per group and then over the groups in a fixed order (no atomics): every output is bitwise repeatable.
+ * A label outside [0, G) gives a NaN loss.  pre and weight fp32 row-major ([B*G, H] and [1, H]), labels int64 [B];
+ * pre, weight, dpre and workspace 16-byte aligned; workspace >= dprb_seqcls_group_ce_workspace_bytes(B, H).  Requires
+ * B >= 1, 2 <= G <= DPRB_SEQCLS_GROUP_MAX, H % 8 == 0, H <= 1024, 0 <= dropout_p < 1 (checked before any launch,
+ * return code 1).  Two launches; never synchronises. */
+#define DPRB_SEQCLS_GROUP_MAX 64
+int64_t dprb_seqcls_group_ce_workspace_bytes(int B, int H);
+int dprb_seqcls_group_ce(const float* pre, const float* weight, const float* bias, const int64_t* labels, int B, int G,
+                         int H, float dropout_p, uint64_t dropout_seed, float* loss, float* logits, void* dpre_bf16,
+                         float* dweight, float* dbias, void* workspace, int64_t workspace_bytes, dprb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Brute-force retrieval : replaces search_index() of
