@@ -99,7 +99,8 @@ class _GroupCE(torch.autograd.Function):
         if drop_in is not None:
             dx.mul_(drop_in)
         g = g.float()
-        return (dx.mul_(g), dw.mul_(g), db.mul_(g), dw_out.mul_(g), db_out.mul_(g), None, None, None, None, None)
+        # dw_out / db_out are saved: scale copies, so a second backward (retain_graph=True) sees them unscaled
+        return (dx.mul_(g), dw.mul_(g), db.mul_(g), dw_out * g, db_out * g, None, None, None, None, None)
 
 
 def _keep_scale(p):
