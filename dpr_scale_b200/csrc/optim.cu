@@ -297,8 +297,9 @@ int adamw_step(float* p, const float* g, float* m, float* v, void* shadow, long 
   DPRB_NUM_SMS(sms);
   AdamArgs a;
   a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.wd = wd;
-  a.bc1 = 1.f - powf(beta1, (float)step);
-  a.bc2_rsqrt = 1.f / sqrtf(1.f - powf(beta2, (float)step));
+  // In double, rounded once: 1 - beta2^step cancels, and fp32 powf would leave a few 1e-6 of error in every update.
+  a.bc1 = (float)(1.0 - pow((double)beta1, step));
+  a.bc2_rsqrt = (float)(1.0 / sqrt(1.0 - pow((double)beta2, step)));
   a.grad_scale = grad_scale; a.max_norm = max_norm;
   adamw_kernel<<<stream_grid(n >> 2, sms), 256, 0, stream>>>(p, g, m, v, (bf16*)shadow, n, a, sumsq);
   DPRB_LAUNCH_CHECK();
