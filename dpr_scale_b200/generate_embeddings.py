@@ -16,12 +16,17 @@ from .trainer import Trainer
 from .utils.config import compose, instantiate
 
 TASK = "dpr_scale_b200.task.dpr_eval_task.GenerateEmbeddingsTask"
-# task=drboost: the same dumps over the concatenated embeddings of the weak encoders
-DRBOOST = "dpr_scale_b200.task.drboost_task.DrBoostTask"
-DRBOOST_DUMPS = {
-    TASK: "dpr_scale_b200.task.drboost_task.DrBoostGenerateEmbeddingsTask",
-    "dpr_scale_b200.task.dpr_eval_task.GenerateQueryEmbeddingsTask":
-        "dpr_scale_b200.task.drboost_task.DrBoostGenerateQueryEmbeddingsTask",
+QUERY_TASK = "dpr_scale_b200.task.dpr_eval_task.GenerateQueryEmbeddingsTask"
+# ensemble tasks (task=drboost, task=spar): the same dumps over the ensemble's concatenated embeddings
+ENSEMBLE_DUMPS = {
+    "dpr_scale_b200.task.drboost_task.DrBoostTask": {
+        TASK: "dpr_scale_b200.task.drboost_task.DrBoostGenerateEmbeddingsTask",
+        QUERY_TASK: "dpr_scale_b200.task.drboost_task.DrBoostGenerateQueryEmbeddingsTask",
+    },
+    "dpr_scale_b200.task.spar_task.SalientPhraseAwareDenseRetrieverTask": {
+        TASK: "dpr_scale_b200.task.spar_task.SparGenerateEmbeddingsTask",
+        QUERY_TASK: "dpr_scale_b200.task.spar_task.SparGenerateQueryEmbeddingsTask",
+    },
 }
 
 
@@ -37,9 +42,7 @@ def run(argv, target):
     init_process_group()
     cfg = compose(name, argv)
     cfg.task.datamodule = None
-    if cfg.task._target_ == DRBOOST:
-        target = DRBOOST_DUMPS[target]
-    cfg.task._target_ = target
+    cfg.task._target_ = ENSEMBLE_DUMPS.get(cfg.task._target_, {}).get(target, target)
     cfg.task.setdefault("checkpoint_path", None)
     task = instantiate(cfg.task, _recursive_=False)
     transform = instantiate(cfg.task.transform)

@@ -8,9 +8,7 @@
 """
 import sys
 
-from .generate_embeddings import run
-
-TASK = "dpr_scale_b200.task.dpr_eval_task.GenerateQueryEmbeddingsTask"
+from .generate_embeddings import QUERY_TASK as TASK, run
 
 
 def main(argv=None):

@@ -16,6 +16,7 @@ Under torchrun the index is sharded over the ranks (each GPU searches the reps_*
 [Q, k] lists; merge) - see search_distributed.  There is no CPU path: without the CUDA library the ops raise DprbError.
 """
 import argparse
+import functools
 import glob
 import json
 import logging
@@ -88,21 +89,34 @@ def search_index(query_embs, corpus_embs, batch, topk, index_offset=0, reference
     return ops.search_topk(q, corpus_embs, topk, index_offset=index_offset, reference_ranking=reference_ranking)
 
 
-def search_segments(q_repr, input_paths, shard, batch, topk, device="cuda", reference_ranking=False):
-    """Search ``shard`` sequential index segments and merge (run_retrieval_pytorch.py:204-230, :272-277)."""
-    assert len(input_paths) % shard == 0, "Invalid Shard number"
-    per = len(input_paths) // shard
-    all_s, all_i, offset = [], [], 0
-    for seg in range(shard):
-        index = build_index(input_paths[seg * per:(seg + 1) * per], device)
-        s, i = search_index(q_repr, index, batch, topk, index_offset=offset, reference_ranking=reference_ranking)
-        offset += index.shape[0]
+def search_loaded(q_repr, loaders, topk, reference_ranking=False):
+    """Search index segments in row order, each built by its loader only when its turn comes (one segment in HBM at a
+    time), and merge the lists -> (scores, row ids counted from the first segment's first row, rows searched)."""
+    all_s, all_i, rows = [], [], 0
+    for load in loaders:
+        index = load()
+        s, i = search_index(q_repr, index, None, topk, index_offset=rows, reference_ranking=reference_ranking)
+        rows += index.shape[0]
         del index
         all_s.append(s)
         all_i.append(i)
-    if shard == 1:
-        return all_s[0], all_i[0]
-    return ops.topk_merge(torch.cat(all_s, dim=1).contiguous(), torch.cat(all_i, dim=1).contiguous(), topk)
+    if len(all_s) == 1:
+        return all_s[0], all_i[0], rows
+    s, i = ops.topk_merge(torch.cat(all_s, dim=1).contiguous(), torch.cat(all_i, dim=1).contiguous(), topk)
+    return s, i, rows
+
+
+def _segment_loaders(input_paths, shard, device):
+    assert len(input_paths) % shard == 0, "Invalid Shard number"
+    per = len(input_paths) // shard
+    return [functools.partial(build_index, input_paths[seg * per:(seg + 1) * per], device) for seg in range(shard)]
+
+
+def search_segments(q_repr, input_paths, shard, batch, topk, device="cuda", reference_ranking=False):
+    """Search ``shard`` sequential index segments and merge (run_retrieval_pytorch.py:204-230, :272-277)."""
+    del batch
+    s, i, _ = search_loaded(q_repr, _segment_loaders(input_paths, shard, device), topk, reference_ranking)
+    return s, i
 
 
 # ------------------------------------------------------------------ multi-GPU: index sharded over ranks
@@ -141,6 +155,16 @@ def gather_rank_lists(scores, indexes):
     return torch.cat(ss, dim=1).contiguous(), torch.cat(ii, dim=1).contiguous()
 
 
+def merge_ranks(scores, indexes, rows, topk):
+    """Every rank's [Q, k] lists over its own ``rows`` -> the global top-k on every rank: rank-local row ids are
+    shifted by the rows of the lower ranks, then one all-gather and ops.topk_merge."""
+    if _world() == 1:
+        return scores, indexes
+    indexes = indexes + global_row_offset(rows, scores.device)
+    gs, gi = gather_rank_lists(scores, indexes)
+    return ops.topk_merge(gs, gi, topk)
+
+
 def search_distributed(q_repr, input_paths, shard, batch, topk, device="cuda", reference_ranking=False):
     """Every rank searches its own block of the index (the reps_{rank} files it wrote in generate_embeddings) and
     the W lists are merged with one all-gather + ops.topk_merge; every rank returns the global result.  The only
@@ -149,24 +173,8 @@ def search_distributed(q_repr, input_paths, shard, batch, topk, device="cuda", r
     if world == 1:
         return search_segments(q_repr, input_paths, shard, batch, topk, device, reference_ranking)
     mine = rank_files(input_paths, dist.get_rank(), world)
-    assert len(mine) % shard == 0, "Invalid Shard number"
-    per = len(mine) // shard
-    all_s, all_i, rows = [], [], 0
-    for seg in range(shard):
-        index = build_index(mine[seg * per:(seg + 1) * per], device)
-        s, i = search_index(q_repr, index, batch, topk, index_offset=rows,    # rank-local row ids for now
-                            reference_ranking=reference_ranking)
-        rows += index.shape[0]
-        del index
-        all_s.append(s)
-        all_i.append(i)
-    s = torch.cat(all_s, dim=1).contiguous()
-    i = torch.cat(all_i, dim=1).contiguous()
-    if shard > 1:
-        s, i = ops.topk_merge(s, i, topk)
-    i = i + global_row_offset(rows, s.device)
-    gs, gi = gather_rank_lists(s, i)
-    return ops.topk_merge(gs, gi, topk)
+    s, i, rows = search_loaded(q_repr, _segment_loaders(mine, shard, device), topk, reference_ranking)
+    return merge_ranks(s, i, rows, topk)
 
 
 # ------------------------------------------------------------------ output (merge_results :96-137, writer :232-300)
