@@ -22,18 +22,23 @@ int check_shape(int nseq, int S, int heads, const char* who) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-int attn_fwd_lse(const void* qkv, const int32_t* attn_mask, void* ctx, float* lse, int nseq, int S, int heads,
-                 float dropout_p, unsigned long long site_seed, cudaStream_t stream) {
+using namespace dprb;
+
+extern "C" int dprb_attn_fwd(const void* qkv, const int32_t* attn_mask, void* ctx, float* lse, int nseq, int S,
+                             int heads, float dropout_p, uint64_t site_seed, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (int rc = check_shape(nseq, S, heads, "attn_fwd")) return rc;
   if (nseq == 0) return 0;
   if (S > SHORT_MAX) return attn_fwd_long(qkv, attn_mask, ctx, lse, nseq, S, heads, dropout_p, site_seed, stream);
   return attn_fwd_wg(qkv, attn_mask, ctx, lse, nseq, S, heads, dropout_p, site_seed, stream);
 }
 
-int attn_bwd_lse(const void* qkv, const int32_t* attn_mask, const void* ctx, const float* lse, const void* dctx,
-                 void* dqkv, float* dbias, int nseq, int S, int heads, float dropout_p,
-                 unsigned long long site_seed, cudaStream_t stream) {
+extern "C" int dprb_attn_bwd(const void* qkv, const int32_t* attn_mask, const void* ctx, const float* lse,
+                             const void* dctx, void* dqkv, float* dbias, int nseq, int S, int heads, float dropout_p,
+                             uint64_t site_seed, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (int rc = check_shape(nseq, S, heads, "attn_bwd")) return rc;
   if (nseq == 0) return 0;
   // D = rowsum(P * dP) is rebuilt in fp32 from Q, K, V, dO and lse; ctx is not read.  The S <= 128 kernel sums the
@@ -43,8 +48,6 @@ int attn_bwd_lse(const void* qkv, const int32_t* attn_mask, const void* ctx, con
   // D = rowsum(dO * ctx) in fp32
   if (int rc = attn_bwd_long(qkv, attn_mask, ctx, lse, dctx, dqkv, nseq, S, heads, dropout_p, site_seed, stream)) return rc;
   // the QKV bias gradient: column sums of the bf16 dQ / dK / dV
-  if (dbias != nullptr) return colsum_bf16(dqkv, 3LL * heads * DH, dbias, nseq * S, 3 * heads * DH, stream);
+  if (dbias != nullptr) return dprb_colsum_bf16(dqkv, 3LL * heads * DH, dbias, nseq * S, 3 * heads * DH, stream);
   return 0;
 }
-
-}  // namespace dprb

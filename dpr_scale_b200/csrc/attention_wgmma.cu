@@ -665,7 +665,7 @@ int attn_bwd_wg(const void* qkv, const int32_t* attn_mask, const float* lse, con
   if (NK == 128) return bwd_short_launch<128>(tq, tdo, attn_mask, lse, dqkv, dbias, nseq, S, heads, drop, stream);
   if (int rc = bwd_launch(tq, tdo, attn_mask, lse, dqkv, nseq, S, heads, drop, stream)) return rc;
   // the QKV bias gradient: column sums of the bf16 dQ / dK / dV
-  return dbias != nullptr ? colsum_bf16(dqkv, 3LL * H, dbias, nseq * S, 3 * H, stream) : 0;
+  return dbias != nullptr ? dprb_colsum_bf16(dqkv, 3LL * H, dbias, nseq * S, 3 * H, stream) : 0;
 }
 
 }  // namespace dprb

@@ -188,8 +188,22 @@ __global__ void add_rows_kernel(bf16* __restrict__ dst, const bf16* __restrict__
 
 }  // namespace
 
-int attn_cls_fwd(const void* qkv, const int32_t* attn_mask, void* ctx_cls, float* probs, int nseq, int S, int heads,
-                 float dropout_p, unsigned long long site_seed, cudaStream_t stream) {
+int add_rows_bf16(void* dst, const void* src, int nrows, int H, long long stride_rows, cudaStream_t stream) {
+  DPRB_REQUIRE(H % 8 == 0, "add_rows: H %% 8 != 0");
+  if (nrows == 0) return 0;
+  const long long n = (long long)nrows * (H / 8);
+  add_rows_kernel<<<(int)((n + 255) / 256), 256, 0, stream>>>((bf16*)dst, (const bf16*)src, nrows, H, stride_rows);
+  DPRB_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace dprb
+
+using namespace dprb;
+
+extern "C" int dprb_attn_cls_fwd(const void* qkv, const int32_t* attn_mask, void* ctx_cls, float* probs, int nseq,
+                                 int S, int heads, float dropout_p, uint64_t site_seed, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(S >= 1 && S <= 512, "attn_cls_fwd: sequence length %d unsupported (1..512)", S);
   if (nseq == 0) return 0;
   const Drop drop = drop_from_site(dropout_p, site_seed);
@@ -202,8 +216,9 @@ int attn_cls_fwd(const void* qkv, const int32_t* attn_mask, void* ctx_cls, float
   return 0;
 }
 
-int attn_cls_bwd(const void* qkv, const float* probs, const void* dctx_cls, void* dqkv, int nseq, int S, int heads,
-                 float dropout_p, unsigned long long site_seed, cudaStream_t stream) {
+extern "C" int dprb_attn_cls_bwd(const void* qkv, const float* probs, const void* dctx_cls, void* dqkv, int nseq,
+                                 int S, int heads, float dropout_p, uint64_t site_seed, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(S >= 1 && S <= 512, "attn_cls_bwd: sequence length %d unsupported (1..512)", S);
   if (nseq == 0) return 0;
   const Drop drop = drop_from_site(dropout_p, site_seed);
@@ -215,14 +230,3 @@ int attn_cls_bwd(const void* qkv, const float* probs, const void* dctx_cls, void
   DPRB_LAUNCH_CHECK();
   return 0;
 }
-
-int add_rows_bf16(void* dst, const void* src, int nrows, int H, long long stride_rows, cudaStream_t stream) {
-  DPRB_REQUIRE(H % 8 == 0, "add_rows: H %% 8 != 0");
-  if (nrows == 0) return 0;
-  const long long n = (long long)nrows * (H / 8);
-  add_rows_kernel<<<(int)((n + 255) / 256), 256, 0, stream>>>((bf16*)dst, (const bf16*)src, nrows, H, stride_rows);
-  DPRB_LAUNCH_CHECK();
-  return 0;
-}
-
-}  // namespace dprb

@@ -18,7 +18,8 @@ namespace dprb {
 typedef __nv_bfloat16 bf16;
 
 // ---------------------------------------------------------------- host-side error plumbing
-void set_last_error(const char* fmt, ...);
+// printf-checked: the entry points format their int64_t parameters with %lld, which needs a (long long) cast
+void set_last_error(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
 #define DPRB_CHECK_CUDA(expr)                                                        \
   do {                                                                               \
     cudaError_t _e = (expr);                                                         \

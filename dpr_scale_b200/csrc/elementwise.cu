@@ -672,10 +672,25 @@ static int check_h(int H, const char* who) {
   return 0;
 }
 
-int embed_ln_fwd(const int64_t* ids, const int64_t* type_ids, const int64_t* pos_ids, const float* word,
-                 const float* pos, const float* type, const float* gamma, const float* beta, void* y, float* stats,
-                 int T, int H, int vocab, int max_pos, int type_vocab, float eps, float dropout_p,
-                 unsigned long long seed, void* y_res, cudaStream_t stream) {
+__global__ void dropout_mask_kernel(uint8_t* out, long long rows, int cols, Drop drop) {
+  const long long n = rows * cols;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const uint32_t r = (uint32_t)(i / cols), c = (uint32_t)(i % cols);
+    float m0, m1;
+    drop.mul2(r, c & ~1u, m0, m1);
+    out[i] = drop.on() ? (uint8_t)(((c & 1u) ? m1 : m0) != 0.f) : (uint8_t)1;
+  }
+}
+
+}  // namespace dprb
+
+using namespace dprb;
+
+extern "C" int dprb_embed_ln_fwd(const int64_t* ids, const int64_t* type_ids, const int64_t* pos_ids, const float* word,
+                                 const float* pos, const float* type, const float* gamma, const float* beta, void* y,
+                                 float* stats, int T, int H, int vocab, int max_pos, int type_vocab, float eps,
+                                 float dropout_p, uint64_t seed, void* y_res, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const Drop drop = make_drop(dropout_p, seed, 0, DROP_SITE_EMBED);
   if (int rc = check_h(H, "embed_ln_fwd")) return rc;
   if (T == 0) return 0;
@@ -689,8 +704,9 @@ int embed_ln_fwd(const int64_t* ids, const int64_t* type_ids, const int64_t* pos
   return 0;
 }
 
-int ln_fwd(const void* z, const float* gamma, const float* beta, void* y, float* stats, float* cls_out,
-           int cls_stride, int T, int H, float eps, int z_f16, void* y_res, cudaStream_t stream) {
+extern "C" int dprb_ln_fwd(const void* z, const float* gamma, const float* beta, void* y, float* stats, float* cls_out,
+                           int cls_stride, int T, int H, float eps, int z_f16, void* y_res, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (int rc = check_h(H, "ln_fwd")) return rc;
   if (T == 0) return 0;
   DPRB_REQUIRE(cls_out == nullptr || cls_stride > 0, "ln_fwd: cls_stride must be positive");
@@ -718,9 +734,10 @@ int ln_fwd(const void* z, const float* gamma, const float* beta, void* y, float*
   return 0;
 }
 
-int ln_bwd(const void* dy, const float* dy_cls, int cls_stride, const void* z, const float* stats,
-           const float* gamma, void* dz, float* dgamma, float* dbeta, float* dbias, int T, int H, void* dzm,
-           float dropout_p, unsigned long long site_seed, int z_f16, cudaStream_t stream) {
+extern "C" int dprb_ln_bwd(const void* dy, const float* dy_cls, int cls_stride, const void* z, const float* stats,
+                           const float* gamma, void* dz, float* dgamma, float* dbeta, float* dbias, int T, int H,
+                           void* dzm, float dropout_p, uint64_t site_seed, int z_f16, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const Drop drop = drop_from_site(dropout_p, site_seed);  // the caller passes the derived site seed
   if (!drop.on()) dzm = nullptr;
   if (int rc = check_h(H, "ln_bwd")) return rc;
@@ -777,10 +794,11 @@ int ln_bwd(const void* dy, const float* dy_cls, int cls_stride, const void* z, c
   return 0;
 }
 
-int embed_ln_bwd(const void* dy, const int64_t* ids, const int64_t* type_ids, const int64_t* pos_ids,
-                 const float* word, const float* pos, const float* type, const float* gamma, const float* stats,
-                 float* dword, float* dpos, float* dtype, float* dgamma, float* dbeta, int T, int H,
-                 float dropout_p, unsigned long long seed, cudaStream_t stream) {
+extern "C" int dprb_embed_ln_bwd(const void* dy, const int64_t* ids, const int64_t* type_ids, const int64_t* pos_ids,
+                                 const float* word, const float* pos, const float* type, const float* gamma,
+                                 const float* stats, float* dword, float* dpos, float* dtype, float* dgamma,
+                                 float* dbeta, int T, int H, float dropout_p, uint64_t seed, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const Drop drop = make_drop(dropout_p, seed, 0, DROP_SITE_EMBED);
   if (int rc = check_h(H, "embed_ln_bwd")) return rc;
   if (T == 0) return 0;
@@ -794,19 +812,14 @@ int embed_ln_bwd(const void* dy, const int64_t* ids, const int64_t* type_ids, co
   return 0;
 }
 
-__global__ void dropout_mask_kernel(uint8_t* out, long long rows, int cols, Drop drop) {
-  const long long n = rows * cols;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const uint32_t r = (uint32_t)(i / cols), c = (uint32_t)(i % cols);
-    float m0, m1;
-    drop.mul2(r, c & ~1u, m0, m1);
-    out[i] = drop.on() ? (uint8_t)(((c & 1u) ? m1 : m0) != 0.f) : (uint8_t)1;
-  }
+extern "C" uint64_t dprb_dropout_site_seed(uint64_t dropout_seed, int layer, int site) {
+  return drop_site_seed64(dropout_seed, layer, site);
 }
 
 // Test aid: materialise the keep mask keep[r * cols + c] of one dropout site (the kernels never store masks).
-int dropout_mask(uint8_t* out, long long rows, int cols, float p, unsigned long long seed, int layer, int site,
-                 cudaStream_t stream) {
+extern "C" int dprb_dropout_mask(uint8_t* out, int64_t rows, int cols, float p, uint64_t seed, int layer, int site,
+                                 dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (rows <= 0 || cols <= 0) return 0;
   const Drop d = make_drop(p, seed, layer, site);
   const long long n = rows * cols;
@@ -815,8 +828,9 @@ int dropout_mask(uint8_t* out, long long rows, int cols, float p, unsigned long 
   return 0;
 }
 
-int colsum_bf16(const void* x, long long ld, float* out, int T, int N, cudaStream_t stream) {
-  DPRB_REQUIRE(N % 8 == 0 && ld % 8 == 0, "colsum: N=%d and ld=%lld must be multiples of 8", N, ld);
+extern "C" int dprb_colsum_bf16(const void* x, int64_t ld, float* out, int T, int N, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DPRB_REQUIRE(N % 8 == 0 && ld % 8 == 0, "colsum: N=%d and ld=%lld must be multiples of 8", N, (long long)ld);
   if (T == 0 || N == 0) return 0;
   DPRB_NUM_SMS(sms);
   const int col_blocks = (N + 255) / 256;
@@ -830,7 +844,8 @@ int colsum_bf16(const void* x, long long ld, float* out, int T, int N, cudaStrea
   return 0;
 }
 
-int gelu_from_pre(const void* pre, void* out, long long n, cudaStream_t stream) {
+extern "C" int dprb_gelu_from_pre(const void* pre, void* out, int64_t n, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(n % 8 == 0 && ((reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
                "gelu_from_pre: n %% 8 == 0 and 16-byte aligned buffers required");
   if (n == 0) return 0;
@@ -841,5 +856,3 @@ int gelu_from_pre(const void* pre, void* out, long long n, cudaStream_t stream) 
   DPRB_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace dprb

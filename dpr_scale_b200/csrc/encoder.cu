@@ -117,16 +117,6 @@ bool prune_last_layer() {
 constexpr int RS_F16 = 1;
 constexpr int X16 = DPRB_GEMM_AUX_F16, O16 = DPRB_GEMM_OUT_F16;
 
-}  // namespace
-
-long long encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S, int save) {
-  Workspace ws;
-  if (plan(w, nseq, S, save, nullptr, &ws)) return -1;
-  return ws.bytes;
-}
-
-namespace {
-
 // The layer stack of both forward entry points.  pooled != nullptr: CLS output (fp32 [nseq, H]), last layer CLS-pruned
 // unless DPRB_NO_CLS_PRUNE is set.  tokens != nullptr: every token of the last layer, bf16 [nseq*S, H], written by the
 // final LayerNorm straight into the caller's buffer; the last layer is never pruned.
@@ -142,9 +132,9 @@ int forward_layers(const dprb_encoder_weights* w, const dprb_encoder_batch* b, f
   const int T = b->nseq * b->S, H = w->hidden, I = w->inter, L = w->layers;
   if (T == 0) return 0;
   const float* ms = w->master;
-  TRY(embed_ln_fwd(b->ids, b->type_ids, b->pos_ids, ms + w->off_word, ms + w->off_pos, ms + w->off_type,
-                   ms + w->off_emb_ln_g, ms + w->off_emb_ln_b, ws.x0, ws.emb_stats, T, H, w->vocab, w->max_pos,
-                   w->type_vocab, w->ln_eps, b->dropout_p, b->dropout_seed, ws.rA, stream));
+  TRY(dprb_embed_ln_fwd(b->ids, b->type_ids, b->pos_ids, ms + w->off_word, ms + w->off_pos, ms + w->off_type,
+                        ms + w->off_emb_ln_g, ms + w->off_emb_ln_b, ws.x0, ws.emb_stats, T, H, w->vocab, w->max_pos,
+                        w->type_vocab, w->ln_eps, b->dropout_p, b->dropout_seed, ws.rA, stream));
   const bf16* x = ws.x0;
   const float dp = b->dropout_p;
   DPRB_REQUIRE(dp >= 0.f && dp < 1.f, "encoder_fwd: dropout_p %f out of range", dp);
@@ -157,44 +147,56 @@ int forward_layers(const dprb_encoder_weights* w, const dprb_encoder_batch* b, f
       // tokens, everything after the attention scores only for the nseq CLS rows (stored in the first nseq rows of
       // this layer's activation buffers; the saved probabilities reuse the lse buffer).
       const int R = b->nseq;
-      TRY(gemm_bf16(x, lw.wqkv, a.qkv, T, 3 * H, H, H, H, 3 * H, 0, 0, DPRB_EPI_BIAS , lw.bqkv, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
-      TRY(attn_cls_fwd(a.qkv, b->attn_mask, a.ctx, a.lse, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
-      TRY(gemm_bf16(a.ctx, lw.wo, a.z1, R, H, H, H, H, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.bo, ws.rA, (long long)b->S * H, nullptr, 1.f, 1, nullptr, dp, site_seed_cls(b, l, DROP_SITE_ATTN_OUT), stream));
-      TRY(ln_fwd(a.z1, lw.ln1g, lw.ln1b, a.x1, a.stats1, nullptr, 1, R, H, w->ln_eps, RS_F16, ws.rB, stream));
-      TRY(gemm_bf16(a.x1, lw.w1, a.hact, R, I, H, H, H, I, 0, 0, GELU_EPI, lw.b1, nullptr, 0, a.hpre, 1.f, 1, nullptr, 0.f, 0, stream));
-      TRY(gemm_bf16(a.hact, lw.w2, a.z2, R, H, I, I, I, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.b2, ws.rB, H, nullptr, 1.f, 1, nullptr, dp, site_seed_cls(b, l, DROP_SITE_FFN_OUT), stream));
-      TRY(ln_fwd(a.z2, lw.ln2g, lw.ln2b, a.out, a.stats2, pooled, 1, R, H, w->ln_eps, RS_F16, nullptr, stream));
+      TRY(dprb_gemm_bf16(x, lw.wqkv, a.qkv, T, 3 * H, H, H, H, 3 * H, 0, 0, DPRB_EPI_BIAS , lw.bqkv, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+      TRY(dprb_attn_cls_fwd(a.qkv, b->attn_mask, a.ctx, a.lse, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
+      TRY(dprb_gemm_bf16(a.ctx, lw.wo, a.z1, R, H, H, H, H, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.bo, ws.rA, (long long)b->S * H, nullptr, 1.f, 1, nullptr, dp, site_seed_cls(b, l, DROP_SITE_ATTN_OUT), stream));
+      TRY(dprb_ln_fwd(a.z1, lw.ln1g, lw.ln1b, a.x1, a.stats1, nullptr, 1, R, H, w->ln_eps, RS_F16, ws.rB, stream));
+      TRY(dprb_gemm_bf16(a.x1, lw.w1, a.hact, R, I, H, H, H, I, 0, 0, GELU_EPI, lw.b1, nullptr, 0, a.hpre, 1.f, 1, nullptr, 0.f, 0, stream));
+      TRY(dprb_gemm_bf16(a.hact, lw.w2, a.z2, R, H, I, I, I, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.b2, ws.rB, H, nullptr, 1.f, 1, nullptr, dp, site_seed_cls(b, l, DROP_SITE_FFN_OUT), stream));
+      TRY(dprb_ln_fwd(a.z2, lw.ln2g, lw.ln2b, a.out, a.stats2, pooled, 1, R, H, w->ln_eps, RS_F16, nullptr, stream));
       x = a.out;
       continue;
     }
-    TRY(gemm_bf16(x, lw.wqkv, a.qkv, T, 3 * H, H, H, H, 3 * H, 0, 0, DPRB_EPI_BIAS , lw.bqkv, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
-    TRY(attn_fwd_lse(a.qkv, b->attn_mask, a.ctx, a.lse, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
-    TRY(gemm_bf16(a.ctx, lw.wo, a.z1, T, H, H, H, H, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.bo, ws.rA, H, nullptr, 1.f, 1, nullptr, dp, site_seed(b, l, DROP_SITE_ATTN_OUT), stream));
-    TRY(ln_fwd(a.z1, lw.ln1g, lw.ln1b, a.x1, a.stats1, nullptr, 1, T, H, w->ln_eps, RS_F16, ws.rB, stream));
-    TRY(gemm_bf16(a.x1, lw.w1, a.hact, T, I, H, H, H, I, 0, 0, GELU_EPI, lw.b1, nullptr, 0, a.hpre, 1.f, 1, nullptr, 0.f, 0, stream));
-    TRY(gemm_bf16(a.hact, lw.w2, a.z2, T, H, I, I, I, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.b2, ws.rB, H, nullptr, 1.f, 1, nullptr, dp, site_seed(b, l, DROP_SITE_FFN_OUT), stream));
+    TRY(dprb_gemm_bf16(x, lw.wqkv, a.qkv, T, 3 * H, H, H, H, 3 * H, 0, 0, DPRB_EPI_BIAS , lw.bqkv, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+    TRY(dprb_attn_fwd(a.qkv, b->attn_mask, a.ctx, a.lse, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
+    TRY(dprb_gemm_bf16(a.ctx, lw.wo, a.z1, T, H, H, H, H, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.bo, ws.rA, H, nullptr, 1.f, 1, nullptr, dp, site_seed(b, l, DROP_SITE_ATTN_OUT), stream));
+    TRY(dprb_ln_fwd(a.z1, lw.ln1g, lw.ln1b, a.x1, a.stats1, nullptr, 1, T, H, w->ln_eps, RS_F16, ws.rB, stream));
+    TRY(dprb_gemm_bf16(a.x1, lw.w1, a.hact, T, I, H, H, H, I, 0, 0, GELU_EPI, lw.b1, nullptr, 0, a.hpre, 1.f, 1, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(a.hact, lw.w2, a.z2, T, H, I, I, I, H, 0, 0, DPRB_EPI_BIAS_RESIDUAL | X16 | O16, lw.b2, ws.rB, H, nullptr, 1.f, 1, nullptr, dp, site_seed(b, l, DROP_SITE_FFN_OUT), stream));
     const bool last = (l == L - 1);
     bf16* y = (last && tokens != nullptr) ? tokens : a.out;
-    TRY(ln_fwd(a.z2, lw.ln2g, lw.ln2b, y, a.stats2, last ? pooled : nullptr, b->S, T, H, w->ln_eps, RS_F16, last ? nullptr : ws.rA, stream));
+    TRY(dprb_ln_fwd(a.z2, lw.ln2g, lw.ln2b, y, a.stats2, last ? pooled : nullptr, b->S, T, H, w->ln_eps, RS_F16, last ? nullptr : ws.rA, stream));
     x = y;
   }
   return 0;
 }
 
 }  // namespace
+}  // namespace dprb
 
-int encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled, cudaStream_t stream) {
-  return forward_layers(w, b, pooled, nullptr, stream);
+using namespace dprb;
+
+extern "C" int64_t dprb_encoder_workspace_bytes(const dprb_encoder_weights* w, int nseq, int S, int save) {
+  Workspace ws;
+  if (plan(w, nseq, S, save, nullptr, &ws)) return -1;
+  return ws.bytes;
 }
 
-int encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_batch* b, void* tokens, cudaStream_t stream) {
+extern "C" int dprb_encoder_fwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, float* pooled,
+                                dprb_stream_t stream) {
+  return forward_layers(w, b, pooled, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int dprb_encoder_fwd_tokens(const dprb_encoder_weights* w, const dprb_encoder_batch* b, void* tokens,
+                                       dprb_stream_t stream) {
   DPRB_REQUIRE(b->save_for_backward == 0, "encoder_fwd_tokens: forward only (save_for_backward must be 0)");
   DPRB_REQUIRE(tokens != nullptr || (long long)b->nseq * b->S == 0, "encoder_fwd_tokens: tokens output is NULL");
-  return forward_layers(w, b, nullptr, reinterpret_cast<bf16*>(tokens), stream);
+  return forward_layers(w, b, nullptr, reinterpret_cast<bf16*>(tokens), static_cast<cudaStream_t>(stream));
 }
 
-int encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, const float* dpooled, int layer_lo,
-                int layer_hi, cudaStream_t stream) {
+extern "C" int dprb_encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, const float* dpooled,
+                                int layer_lo, int layer_hi, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   Workspace ws;
   DPRB_REQUIRE(b->save_for_backward, "encoder_bwd: forward was run without save_for_backward");
   DPRB_REQUIRE(w->grads != nullptr, "encoder_bwd: grads arena is NULL");
@@ -214,63 +216,61 @@ int encoder_bwd(const dprb_encoder_weights* w, const dprb_encoder_batch* b, cons
     const bf16* gLin = dp > 0.f ? ws.gB2 : ws.gB;
     if (last && prune_last_layer()) {
       const int R = b->nseq;
-      TRY(ln_bwd(nullptr, dpooled, 1, a.z2, a.stats2, lw.ln2g, ws.gB, lw.g_ln2g, lw.g_ln2b, lw.g_b2, R, H, ws.gB2, dp,
-                 site_seed_cls(b, l, DROP_SITE_FFN_OUT), RS_F16, stream));
-      TRY(gemm_bf16(gLin, a.hact, lw.g_w2, H, I, R, H, I, I, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
-      TRY(gemm_bf16(gLin, lw.w2, ws.gH, R, I, H, H, I, I, 0, 1, DGELU_EPI, nullptr, a.hpre, I, nullptr, 1.f, 1, lw.g_b1, 0.f, 0, stream));
-      TRY(gemm_bf16(ws.gH, a.x1, lw.g_w1, I, H, R, I, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
-      TRY(gemm_bf16(ws.gH, lw.w1, ws.gA, R, H, I, I, H, H, 0, 1, DPRB_EPI_BIAS_RESIDUAL, nullptr, ws.gB, H, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
-      TRY(ln_bwd(ws.gA, nullptr, 1, a.z1, a.stats1, lw.ln1g, ws.gB, lw.g_ln1g, lw.g_ln1b, lw.g_bo, R, H, ws.gB2, dp,
-                 site_seed_cls(b, l, DROP_SITE_ATTN_OUT), RS_F16, stream));
-      TRY(gemm_bf16(gLin, a.ctx, lw.g_wo, H, H, R, H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
-      TRY(gemm_bf16(gLin, lw.wo, ws.gA, R, H, H, H, H, H, 0, 1, DPRB_EPI_BIAS, nullptr, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
-      TRY(attn_cls_bwd(a.qkv, a.lse, ws.gA, ws.gQKV, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
-      TRY(colsum_bf16(ws.gQKV, 3 * H, lw.g_bqkv, T, 3 * H, stream));
-      TRY(gemm_bf16(ws.gQKV, x, lw.g_wqkv, 3 * H, H, T, 3 * H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+      TRY(dprb_ln_bwd(nullptr, dpooled, 1, a.z2, a.stats2, lw.ln2g, ws.gB, lw.g_ln2g, lw.g_ln2b, lw.g_b2, R, H, ws.gB2, dp,
+                      site_seed_cls(b, l, DROP_SITE_FFN_OUT), RS_F16, stream));
+      TRY(dprb_gemm_bf16(gLin, a.hact, lw.g_w2, H, I, R, H, I, I, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+      TRY(dprb_gemm_bf16(gLin, lw.w2, ws.gH, R, I, H, H, I, I, 0, 1, DGELU_EPI, nullptr, a.hpre, I, nullptr, 1.f, 1, lw.g_b1, 0.f, 0, stream));
+      TRY(dprb_gemm_bf16(ws.gH, a.x1, lw.g_w1, I, H, R, I, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+      TRY(dprb_gemm_bf16(ws.gH, lw.w1, ws.gA, R, H, I, I, H, H, 0, 1, DPRB_EPI_BIAS_RESIDUAL, nullptr, ws.gB, H, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+      TRY(dprb_ln_bwd(ws.gA, nullptr, 1, a.z1, a.stats1, lw.ln1g, ws.gB, lw.g_ln1g, lw.g_ln1b, lw.g_bo, R, H, ws.gB2, dp,
+                      site_seed_cls(b, l, DROP_SITE_ATTN_OUT), RS_F16, stream));
+      TRY(dprb_gemm_bf16(gLin, a.ctx, lw.g_wo, H, H, R, H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+      TRY(dprb_gemm_bf16(gLin, lw.wo, ws.gA, R, H, H, H, H, H, 0, 1, DPRB_EPI_BIAS, nullptr, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+      TRY(dprb_attn_cls_bwd(a.qkv, a.lse, ws.gA, ws.gQKV, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
+      TRY(dprb_colsum_bf16(ws.gQKV, 3 * H, lw.g_bqkv, T, 3 * H, stream));
+      TRY(dprb_gemm_bf16(ws.gQKV, x, lw.g_wqkv, 3 * H, H, T, 3 * H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
       // dx = dqkv Wqkv, plus the residual gradient dz1 on the CLS rows only
-      TRY(gemm_bf16(ws.gQKV, lw.wqkv, ws.gA, T, H, 3 * H, 3 * H, H, H, 0, 1, DPRB_EPI_BIAS, nullptr, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+      TRY(dprb_gemm_bf16(ws.gQKV, lw.wqkv, ws.gA, T, H, 3 * H, 3 * H, H, H, 0, 1, DPRB_EPI_BIAS, nullptr, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
       TRY(add_rows_bf16(ws.gA, ws.gB, R, H, b->S, stream));
       continue;
     }
     // LN2 backward (+ db2)
-    TRY(ln_bwd(last ? nullptr : ws.gA, last ? dpooled : nullptr, b->S, a.z2, a.stats2, lw.ln2g, ws.gB, lw.g_ln2g,
-               lw.g_ln2b, lw.g_b2, T, H, ws.gB2, dp, site_seed(b, l, DROP_SITE_FFN_OUT), RS_F16, stream));
+    TRY(dprb_ln_bwd(last ? nullptr : ws.gA, last ? dpooled : nullptr, b->S, a.z2, a.stats2, lw.ln2g, ws.gB, lw.g_ln2g,
+                    lw.g_ln2b, lw.g_b2, T, H, ws.gB2, dp, site_seed(b, l, DROP_SITE_FFN_OUT), RS_F16, stream));
     // lean activations: the GELU output was not kept - rebuild it from the saved pre-activation
-    if (ws.lean) TRY(gelu_from_pre(a.hpre, a.hact, (long long)T * I, stream));
+    if (ws.lean) TRY(dprb_gelu_from_pre(a.hpre, a.hact, (long long)T * I, stream));
     // dW2 += dz2^T hact
-    TRY(gemm_bf16(gLin, a.hact, lw.g_w2, H, I, T, H, I, I, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(gLin, a.hact, lw.g_w2, H, I, T, H, I, I, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
     // dhpre = (dz2 W2) * gelu'(hpre)
-    TRY(gemm_bf16(gLin, lw.w2, ws.gH, T, I, H, H, I, I, 0, 1, DGELU_EPI, nullptr, a.hpre, I, nullptr, 1.f, 1, lw.g_b1, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(gLin, lw.w2, ws.gH, T, I, H, H, I, I, 0, 1, DGELU_EPI, nullptr, a.hpre, I, nullptr, 1.f, 1, lw.g_b1, 0.f, 0, stream));
     // (db1 = column sums of dhpre is fused into that epilogue: +58 us vs 129 us for a separate streaming pass)
     // dW1 += dhpre^T x1
-    TRY(gemm_bf16(ws.gH, a.x1, lw.g_w1, I, H, T, I, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(ws.gH, a.x1, lw.g_w1, I, H, T, I, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
     // dx1 = dhpre W1 + dz2
-    TRY(gemm_bf16(ws.gH, lw.w1, ws.gA, T, H, I, I, H, H, 0, 1, DPRB_EPI_BIAS_RESIDUAL, nullptr, ws.gB, H, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(ws.gH, lw.w1, ws.gA, T, H, I, I, H, H, 0, 1, DPRB_EPI_BIAS_RESIDUAL, nullptr, ws.gB, H, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
     // LN1 backward (+ dbo)
-    TRY(ln_bwd(ws.gA, nullptr, 1, a.z1, a.stats1, lw.ln1g, ws.gB, lw.g_ln1g, lw.g_ln1b, lw.g_bo, T, H, ws.gB2, dp,
-               site_seed(b, l, DROP_SITE_ATTN_OUT), RS_F16, stream));
+    TRY(dprb_ln_bwd(ws.gA, nullptr, 1, a.z1, a.stats1, lw.ln1g, ws.gB, lw.g_ln1g, lw.g_ln1b, lw.g_bo, T, H, ws.gB2, dp,
+                    site_seed(b, l, DROP_SITE_ATTN_OUT), RS_F16, stream));
     // lean activations: the attention output was not kept - one more attention forward (same dropout stream)
-    if (ws.lean) TRY(attn_fwd_lse(a.qkv, b->attn_mask, a.ctx, a.lse, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
+    if (ws.lean) TRY(dprb_attn_fwd(a.qkv, b->attn_mask, a.ctx, a.lse, b->nseq, b->S, w->heads, dp, site_seed(b, l, DROP_SITE_ATTN), stream));
     // dWo += dz1^T ctx
-    TRY(gemm_bf16(gLin, a.ctx, lw.g_wo, H, H, T, H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(gLin, a.ctx, lw.g_wo, H, H, T, H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
     // dctx = dz1 Wo
-    TRY(gemm_bf16(gLin, lw.wo, ws.gA, T, H, H, H, H, H, 0, 1, DPRB_EPI_BIAS, nullptr, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(gLin, lw.wo, ws.gA, T, H, H, H, H, H, 0, 1, DPRB_EPI_BIAS, nullptr, nullptr, 0, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
     // (+ dbqkv: column sums of dqkv fused into the attention-backward epilogue)
-    TRY(attn_bwd_lse(a.qkv, b->attn_mask, a.ctx, a.lse, ws.gA, ws.gQKV, lw.g_bqkv, b->nseq, b->S, w->heads, dp,
-                     site_seed(b, l, DROP_SITE_ATTN), stream));
+    TRY(dprb_attn_bwd(a.qkv, b->attn_mask, a.ctx, a.lse, ws.gA, ws.gQKV, lw.g_bqkv, b->nseq, b->S, w->heads, dp,
+                      site_seed(b, l, DROP_SITE_ATTN), stream));
     // dWqkv += dqkv^T x
-    TRY(gemm_bf16(ws.gQKV, x, lw.g_wqkv, 3 * H, H, T, 3 * H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(ws.gQKV, x, lw.g_wqkv, 3 * H, H, T, 3 * H, H, H, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0, nullptr, 1.f, 0, nullptr, 0.f, 0, stream));
     // dx = dqkv Wqkv + dz1
-    TRY(gemm_bf16(ws.gQKV, lw.wqkv, ws.gA, T, H, 3 * H, 3 * H, H, H, 0, 1, DPRB_EPI_BIAS_RESIDUAL, nullptr, ws.gB, H, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
+    TRY(dprb_gemm_bf16(ws.gQKV, lw.wqkv, ws.gA, T, H, 3 * H, 3 * H, H, H, 0, 1, DPRB_EPI_BIAS_RESIDUAL, nullptr, ws.gB, H, nullptr, 1.f, 1, nullptr, 0.f, 0, stream));
   }
   if (layer_lo == 0) {
     const float* ms = w->master;
     float* gr = w->grads;
-    TRY(embed_ln_bwd(ws.gA, b->ids, b->type_ids, b->pos_ids, ms + w->off_word, ms + w->off_pos, ms + w->off_type,
-                     ms + w->off_emb_ln_g, ws.emb_stats, gr + w->off_word, gr + w->off_pos, gr + w->off_type,
-                     gr + w->off_emb_ln_g, gr + w->off_emb_ln_b, T, H, b->dropout_p, b->dropout_seed, stream));
+    TRY(dprb_embed_ln_bwd(ws.gA, b->ids, b->type_ids, b->pos_ids, ms + w->off_word, ms + w->off_pos, ms + w->off_type,
+                          ms + w->off_emb_ln_g, ws.emb_stats, gr + w->off_word, gr + w->off_pos, gr + w->off_type,
+                          gr + w->off_emb_ln_g, gr + w->off_emb_ln_b, T, H, b->dropout_p, b->dropout_seed, stream));
   }
   return 0;
 }
-
-}  // namespace dprb

@@ -231,18 +231,23 @@ Layout carve(void* ws, long long total, int tiles) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-long long expert_group_workspace_bytes(int N, int S, int K) {
+using namespace dprb;
+
+extern "C" int64_t dprb_expert_group_workspace_bytes(int N, int S, int K) {
   if (N < 1 || S < 1 || K < 1) return 0;
   const long long total = (long long)N * S * K;
   if (total >= (1LL << 31)) return -1;
   return carve(nullptr, total, (int)((total + TILE - 1) / TILE)).bytes;
 }
 
-int expert_group(const int32_t* ids, const float* w, const int32_t* mask, const int32_t* tokens, const void* reps,
-                 long long ldr, int N, int S, int K, int P, int V, float threshold, int flags, int32_t* count,
-                 int32_t* out_expert, int32_t* out_seq, int32_t* out_tok, float* out_w, float* out_payload,
-                 void* workspace, long long workspace_bytes, cudaStream_t stream) {
+extern "C" int dprb_expert_group(const int32_t* ids, const float* w, const int32_t* mask, const int32_t* tokens,
+                                 const void* reps, int64_t ldr, int N, int S, int K, int P, int V, float threshold,
+                                 int flags, int32_t* count, int32_t* out_expert, int32_t* out_seq, int32_t* out_tok,
+                                 float* out_w, float* out_payload, void* workspace, int64_t workspace_bytes,
+                                 dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool ctx_id = (flags & DPRB_EXPERT_GROUP_CONTEXT_ID) != 0;
   const bool per_seq = (flags & DPRB_EXPERT_GROUP_PER_SEQUENCE) != 0;
   DPRB_REQUIRE((flags & ~(DPRB_EXPERT_GROUP_CONTEXT_ID | DPRB_EXPERT_GROUP_PER_SEQUENCE)) == 0,
@@ -261,7 +266,7 @@ int expert_group(const int32_t* ids, const float* w, const int32_t* mask, const 
     DPRB_REQUIRE(P % 8 == 0 && P >= 8 && P <= MAX_P, "expert_group: P=%d unsupported (multiple of 8, 8 .. %d)", P,
                  MAX_P);
     DPRB_REQUIRE(reps != nullptr && ldr >= P && ldr % 8 == 0, "expert_group: reps NULL or ldr=%lld (>= P=%d, multiple "
-                 "of 8)", ldr, P);
+                 "of 8)", (long long)ldr, P);
     DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(reps) | reinterpret_cast<uintptr_t>(out_payload)) & 15) == 0,
                  "expert_group: reps / payload must be 16-byte aligned");
   }
@@ -269,7 +274,7 @@ int expert_group(const int32_t* ids, const float* w, const int32_t* mask, const 
   const Layout l = carve(workspace, total, tiles);
   DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= l.bytes,
                "expert_group: workspace of %lld bytes, %lld needed (dprb_expert_group_workspace_bytes)",
-               workspace_bytes, l.bytes);
+               (long long)workspace_bytes, l.bytes);
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "expert_group: workspace must be 256-byte aligned");
   DPRB_NUM_SMS(sms);
 
@@ -308,5 +313,3 @@ int expert_group(const int32_t* ids, const float* w, const int32_t* mask, const 
   DPRB_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace dprb

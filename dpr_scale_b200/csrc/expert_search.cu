@@ -185,28 +185,36 @@ expert_search_kernel(const SearchParams p) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-int expert_search_block_queries(long long N) { return fixed_acc_block_queries(N); }
+using namespace dprb;
 
-long long expert_search_workspace_bytes(long long N, int Qb) { return fixed_acc_workspace_bytes(N, Qb); }
+extern "C" int dprb_expert_search_block_queries(int64_t N) { return fixed_acc_block_queries(N); }
 
-int expert_search(const void* payload, const int32_t* row, const int32_t* tile_bounds, long long E, int T, int P,
-                  int ldp, const void* cls, int Pc, int ldc, const long long* row_ids, long long N,
-                  const void* q_payload, const int32_t* q_seq, long long Eq, const void* q_cls, int Qb,
-                  const int32_t* groups, const int32_t* item_end, int G, int items, int k, float* out_scores,
-                  long long* out_ids, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+extern "C" int64_t dprb_expert_search_workspace_bytes(int64_t N, int Qb) { return fixed_acc_workspace_bytes(N, Qb); }
+
+extern "C" int dprb_expert_search(const void* payload, const int32_t* row, const int32_t* tile_bounds, int64_t E, int T,
+                                  int P, int ldp, const void* cls, int Pc, int ldc, const int64_t* row_ids_, int64_t N,
+                                  const void* q_payload, const int32_t* q_seq, int64_t Eq, const void* q_cls, int Qb,
+                                  const int32_t* groups, const int32_t* item_end, int G, int items, int k,
+                                  float* out_scores, int64_t* out_ids_, void* workspace, int64_t workspace_bytes,
+                                  dprb_stream_t stream_) {
+  const long long* row_ids = reinterpret_cast<const long long*>(row_ids_);
+  long long* out_ids = reinterpret_cast<long long*>(out_ids_);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(P % 8 == 0 && P >= 8 && P <= MAX_P && ldp >= P && ldp % 8 == 0,
                "expert_search: P=%d ldp=%d unsupported (P a multiple of 8, 8 .. %d; ldp >= P, a multiple of 8)", P,
                ldp, MAX_P);
-  DPRB_REQUIRE(N >= 1 && N < (1LL << 31), "expert_search: N=%lld passages outside [1, 2^31)", N);
+  DPRB_REQUIRE(N >= 1 && N < (1LL << 31), "expert_search: N=%lld passages outside [1, 2^31)", (long long)N);
   DPRB_REQUIRE(E >= 0 && E < (1LL << 31) && Eq >= 0 && Eq < (1LL << 31),
-               "expert_search: E=%lld index entries or Eq=%lld query entries outside [0, 2^31)", E, Eq);
+               "expert_search: E=%lld index entries or Eq=%lld query entries outside [0, 2^31)", (long long)E,
+               (long long)Eq);
   DPRB_REQUIRE(T >= 0 && G >= 0 && items >= 0 && (G > 0 || items == 0),
                "expert_search: T=%d tiles, G=%d groups, %d work items", T, G, items);
-  DPRB_REQUIRE(k >= 1 && k <= 1024 && k <= N, "expert_search: k=%d outside [1, min(1024, N=%lld)]", k, N);
-  DPRB_REQUIRE(Qb >= 1 && Qb <= expert_search_block_queries(N),
+  DPRB_REQUIRE(k >= 1 && k <= 1024 && k <= N, "expert_search: k=%d outside [1, min(1024, N=%lld)]", k, (long long)N);
+  DPRB_REQUIRE(Qb >= 1 && Qb <= dprb_expert_search_block_queries(N),
                "expert_search: Qb=%d queries per block outside [1, %d] (dprb_expert_search_block_queries)", Qb,
-               expert_search_block_queries(N));
+               dprb_expert_search_block_queries(N));
   DPRB_REQUIRE((cls == nullptr) == (q_cls == nullptr), "expert_search: give both CLS operands or neither");
   if (cls != nullptr)
     DPRB_REQUIRE(Pc % 8 == 0 && Pc >= 8 && Pc <= MAX_P && ldc >= Pc && ldc % 8 == 0,
@@ -220,9 +228,9 @@ int expert_search(const void* payload, const int32_t* row, const int32_t* tile_b
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(payload) | reinterpret_cast<uintptr_t>(q_payload) |
                  reinterpret_cast<uintptr_t>(cls) | reinterpret_cast<uintptr_t>(q_cls)) & 15) == 0,
                "expert_search: payloads must be 16-byte aligned");
-  const long long need = expert_search_workspace_bytes(N, Qb);
+  const long long need = dprb_expert_search_workspace_bytes(N, Qb);
   DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= need && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
-               "expert_search: workspace of %lld bytes (256-byte aligned), %lld needed", workspace_bytes, need);
+               "expert_search: workspace of %lld bytes (256-byte aligned), %lld needed", (long long)workspace_bytes, need);
   DPRB_NUM_SMS(sms);
 
   FixedAcc fa;
@@ -254,5 +262,3 @@ int expert_search(const void* payload, const int32_t* row, const int32_t* tile_b
   }
   return fixed_acc_select(fa.acc, N, Qb, k, row_ids, out_scores, out_ids, stream);
 }
-
-}  // namespace dprb

@@ -455,11 +455,15 @@ int choose_splits(int tiles, int k_blocks, int sms) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long long lda, long long ldb,
-              long long ldd, int a_mn_major, int b_mn_major, int epilogue, const float* bias, const void* aux,
-              long long ld_aux, void* out2, float alpha, int splits, float* colsum, float dropout_p,
-              unsigned long long drop_site_seed, cudaStream_t stream) {
+using namespace dprb;
+
+extern "C" int dprb_gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, int64_t lda, int64_t ldb,
+                              int64_t ldd, int a_mn_major, int b_mn_major, int epilogue, const float* bias,
+                              const void* aux, int64_t ld_aux, void* out2, float alpha, int splits, float* colsum,
+                              float dropout_p, uint64_t drop_site_seed, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
   const int dt_flags = epilogue & ~0xFF;   // DPRB_GEMM_{A,B,AUX,OUT}_F16, DPRB_GEMM_SAVE_PRE
   epilogue &= 0xFF;
@@ -473,9 +477,9 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   DPRB_REQUIRE(!out_f16 || colsum == nullptr, "gemm: colsum reads a bf16 slab (not available with fp16 output)");
   const bool f32_out = (epilogue == DPRB_EPI_F32_ATOMIC_ADD || epilogue == DPRB_EPI_F32_STORE);
   DPRB_REQUIRE(f32_out || (ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0),
-               "gemm: bf16 output must be 16-byte aligned with ldd %% 8 == 0 (ldd=%lld)", ldd);
+               "gemm: bf16 output must be 16-byte aligned with ldd %% 8 == 0 (ldd=%lld)", (long long)ldd);
   DPRB_REQUIRE(!f32_out || (ldd % 4 == 0 && (reinterpret_cast<uintptr_t>(D) & 15) == 0),
-               "gemm: fp32 output must be 16-byte aligned with ldd %% 4 == 0 (ldd=%lld)", ldd);
+               "gemm: fp32 output must be 16-byte aligned with ldd %% 4 == 0 (ldd=%lld)", (long long)ldd);
   const bool has_aux = epilogue == DPRB_EPI_BIAS_RESIDUAL || epilogue == DPRB_EPI_DGELU || epilogue == DPRB_EPI_DGELU_PRE;
   if (has_aux)
     DPRB_REQUIRE(aux != nullptr && ld_aux % 8 == 0 && (reinterpret_cast<uintptr_t>(aux) & 15) == 0,
@@ -556,7 +560,7 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, long l
   }
 }
 
-int gemm_profile_enable(int enable, int max_launches) {
+extern "C" int dprb_gemm_profile_enable(int enable, int max_launches) {
   if (enable) {
     const size_t want = (size_t)max_launches * 2;
     while (g_prof.ev.size() < want) {
@@ -572,7 +576,7 @@ int gemm_profile_enable(int enable, int max_launches) {
 }
 
 // Sums the recorded launch durations (synchronises on each end event). Outputs: total ms, total FLOPs, launches.
-int gemm_profile_read(double* total_ms, double* total_flops, long long* launches) {
+extern "C" int dprb_gemm_profile_read(double* total_ms, double* total_flops, int64_t* launches) {
   double ms = 0.0, fl = 0.0;
   for (size_t i = 0; i + 1 < g_prof.used; i += 2) {
     DPRB_CHECK_CUDA(cudaEventSynchronize(g_prof.ev[i + 1]));
@@ -583,8 +587,6 @@ int gemm_profile_read(double* total_ms, double* total_flops, long long* launches
   }
   if (total_ms) *total_ms = ms;
   if (total_flops) *total_flops = fl;
-  if (launches) *launches = (long long)(g_prof.used / 2);
+  if (launches) *launches = (int64_t)(g_prof.used / 2);
   return 0;
 }
-
-}  // namespace dprb

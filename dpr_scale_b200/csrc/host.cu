@@ -1,9 +1,24 @@
-// Host plumbing shared by the kernel files: the SM count and the one TMA tensor-map encoder.
+// Host plumbing shared by the kernel files: the thread-local error string, the launch counter, the SM count and the one
+// TMA tensor-map encoder, plus the C entry points that report them.
 #include <atomic>
+#include <cstdarg>
+#include <cstdio>
 #include "common.cuh"
 #include "dprb_internal.h"
 
 namespace dprb {
+
+static thread_local char g_err[1024] = "";
+
+void set_last_error(const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(g_err, sizeof(g_err), fmt, ap);
+  va_end(ap);
+}
+
+static std::atomic<long long> g_launches{0};
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 int num_sms() {
   static std::atomic<int> cached{0};
@@ -57,3 +72,8 @@ int encode_tmap(CUtensorMap* out, const char* what, CUtensorMapDataType dtype, i
 }
 
 }  // namespace dprb
+
+extern "C" int dprb_version(void) { return DPRB_VERSION; }
+extern "C" const char* dprb_last_error(void) { return dprb::g_err; }
+extern "C" int dprb_num_sms(void) { return dprb::num_sms(); }
+extern "C" int64_t dprb_launch_count(void) { return dprb::g_launches.load(std::memory_order_relaxed); }

@@ -374,10 +374,29 @@ int make_tmap_tokens(CUtensorMap* out, const void* base, long long n, int S, int
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
-}  // namespace
+template <int KQ_MAX>
+int launch_maxsim_expert(const CUtensorMap& tq, const CUtensorMap& td, const MaxSimExpertParams& prm, int B,
+                         cudaStream_t stream) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    DPRB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_expert_kernel<KQ_MAX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         EXPERT_SMEM_BYTES));
+    attr_done = true;
+  }
+  maxsim_expert_kernel<KQ_MAX><<<(unsigned)B, THREADS, EXPERT_SMEM_BYTES, stream>>>(tq, td, prm);
+  DPRB_LAUNCH_CHECK();
+  return 0;
+}
 
-int maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_t* d_mask, const int32_t* q_index,
-               int nq, int SQ, int B, int SD, int P, int pool, float* score, cudaStream_t stream) {
+}  // namespace
+}  // namespace dprb
+
+using namespace dprb;
+
+extern "C" int dprb_maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_t* d_mask,
+                               const int32_t* q_index, int nq, int SQ, int B, int SD, int P, int pool, float* score,
+                               dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(P % 8 == 0 && P >= 8 && P <= 1024, "maxsim_fwd: P=%d unsupported (multiple of 8, at most 1024)", P);
   DPRB_REQUIRE(SQ >= 2 && SQ <= MAX_S && SD >= 2 && SD <= MAX_S,
                "maxsim_fwd: sequence lengths SQ=%d SD=%d unsupported (2 .. 512, token 0 is skipped)", SQ, SD);
@@ -403,25 +422,11 @@ int maxsim_fwd(const void* q, const void* d, const int32_t* q_mask, const int32_
   return 0;
 }
 
-namespace {
-template <int KQ_MAX>
-int launch_maxsim_expert(const CUtensorMap& tq, const CUtensorMap& td, const MaxSimExpertParams& prm, int B,
-                         cudaStream_t stream) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    DPRB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_expert_kernel<KQ_MAX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         EXPERT_SMEM_BYTES));
-    attr_done = true;
-  }
-  maxsim_expert_kernel<KQ_MAX><<<(unsigned)B, THREADS, EXPERT_SMEM_BYTES, stream>>>(tq, td, prm);
-  DPRB_LAUNCH_CHECK();
-  return 0;
-}
-}  // namespace
-
-int maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const float* q_w, const int32_t* d_ids,
-                      const float* d_w, const void* q_cls, const void* d_cls, const int32_t* q_index, int nq, int SQ,
-                      int B, int SD, int P, int KQ, int KD, int Pc, int pool, float* score, cudaStream_t stream) {
+extern "C" int dprb_maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const float* q_w,
+                                      const int32_t* d_ids, const float* d_w, const void* q_cls, const void* d_cls,
+                                      const int32_t* q_index, int nq, int SQ, int B, int SD, int P, int KQ, int KD,
+                                      int Pc, int pool, float* score, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(P % 8 == 0 && P >= 8 && P <= 1024, "maxsim_expert_fwd: P=%d unsupported (multiple of 8, at most 1024)",
                P);
   DPRB_REQUIRE(SQ >= 2 && SQ <= MAX_S && SD >= 2 && SD <= MAX_S,
@@ -455,5 +460,3 @@ int maxsim_expert_fwd(const void* q, const void* d, const int32_t* q_ids, const 
   if (KQ <= 4) return launch_maxsim_expert<4>(tq, td, prm, B, stream);
   return launch_maxsim_expert<8>(tq, td, prm, B, stream);
 }
-
-}  // namespace dprb

@@ -276,8 +276,12 @@ int stream_grid(long long n4, int sms) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-int sumsq_f32(const float* g, long long n, float* out, cudaStream_t stream) {
+using namespace dprb;
+
+extern "C" int dprb_sumsq_f32(const float* g, int64_t n, float* out, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(n >= 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0, "sumsq: buffer must be 16-byte aligned");
   if (n == 0) return 0;
   DPRB_NUM_SMS(sms);
@@ -286,9 +290,10 @@ int sumsq_f32(const float* g, long long n, float* out, cudaStream_t stream) {
   return 0;
 }
 
-int adamw_step(float* p, const float* g, float* m, float* v, void* shadow, long long n, float lr, float beta1,
-               float beta2, float eps, float wd, int step, float grad_scale, const float* sumsq, float max_norm,
-               cudaStream_t stream) {
+extern "C" int dprb_adamw_step(float* p, const float* g, float* m, float* v, void* shadow, int64_t n, float lr,
+                               float beta1, float beta2, float eps, float wd, int step, float grad_scale,
+                               const float* sumsq, float max_norm, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(step >= 1, "adamw_step: step must start at 1 (got %d)", step);
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                  reinterpret_cast<uintptr_t>(v)) & 15) == 0 && (reinterpret_cast<uintptr_t>(shadow) & 7) == 0,
@@ -306,17 +311,20 @@ int adamw_step(float* p, const float* g, float* m, float* v, void* shadow, long 
   return 0;
 }
 
-long long lamb_workspace_bytes(int nchunks, int nseg) {
+extern "C" int64_t dprb_lamb_workspace_bytes(int nchunks, int nseg) {
   if (nchunks < 1 || nseg < 1) return -1;
   return ((2LL * nchunks + nseg) * (long long)sizeof(float) + 255) & ~255LL;
 }
 
-int lamb_step(float* p, const float* g, float* m, float* v, void* shadow, long long n, const long long* plan,
-              int nchunks, int nseg, float lr, float beta1, float beta2, float eps, float wd, float clamp_value,
-              int adam, int debias, int step, float grad_scale, const float* sumsq, float max_norm, void* workspace,
-              long long workspace_bytes, cudaStream_t stream) {
+extern "C" int dprb_lamb_step(float* p, const float* g, float* m, float* v, void* shadow, int64_t n,
+                              const int64_t* plan_, int nchunks, int nseg, float lr, float beta1, float beta2,
+                              float eps, float wd, float clamp_value, int adam, int debias, int step, float grad_scale,
+                              const float* sumsq, float max_norm, void* workspace, int64_t workspace_bytes,
+                              dprb_stream_t stream_) {
+  const long long* plan = reinterpret_cast<const long long*>(plan_);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(step >= 1, "lamb_step: step must start at 1 (got %d)", step);
-  DPRB_REQUIRE(n >= 0 && (n & 3) == 0, "lamb_step: arena length must be a multiple of 4 (got %lld)", n);
+  DPRB_REQUIRE(n >= 0 && (n & 3) == 0, "lamb_step: arena length must be a multiple of 4 (got %lld)", (long long)n);
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                  reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(shadow) & 7) == 0 && (reinterpret_cast<uintptr_t>(plan) & 7) == 0,
@@ -324,9 +332,9 @@ int lamb_step(float* p, const float* g, float* m, float* v, void* shadow, long l
   if (n == 0) return 0;
   DPRB_REQUIRE(plan != nullptr && nchunks >= nseg && nseg >= 1, "lamb_step: need a plan with 1 <= nseg <= nchunks "
                "(got nchunks %d, nseg %d)", nchunks, nseg);
-  DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= lamb_workspace_bytes(nchunks, nseg),
-               "lamb_step: workspace of %lld bytes is smaller than dprb_lamb_workspace_bytes = %lld", workspace_bytes,
-               lamb_workspace_bytes(nchunks, nseg));
+  DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= dprb_lamb_workspace_bytes(nchunks, nseg),
+               "lamb_step: workspace of %lld bytes is smaller than dprb_lamb_workspace_bytes = %lld",
+               (long long)workspace_bytes, (long long)dprb_lamb_workspace_bytes(nchunks, nseg));
   DPRB_NUM_SMS(sms);
   LambArgs a;
   a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.wd = wd; a.clamp_value = clamp_value; a.adam = adam != 0;
@@ -345,9 +353,10 @@ int lamb_step(float* p, const float* g, float* m, float* v, void* shadow, long l
   return 0;
 }
 
-int madgrad_step(float* p, const float* g, float* nu, float* s, const float* x0, void* shadow, long long n, float lr,
-                 float momentum, float wd, float eps, int k, float grad_scale, const float* sumsq, float max_norm,
-                 cudaStream_t stream) {
+extern "C" int dprb_madgrad_step(float* p, const float* g, float* nu, float* s, const float* x0, void* shadow,
+                                 int64_t n, float lr, float momentum, float wd, float eps, int k, float grad_scale,
+                                 const float* sumsq, float max_norm, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(k >= 0, "madgrad_step: k counts steps from 0 (got %d)", k);
   DPRB_REQUIRE(momentum >= 0.f && momentum < 1.f, "madgrad_step: momentum must be in [0, 1) (got %g)", momentum);
   DPRB_REQUIRE((momentum == 0.f) == (x0 == nullptr), "madgrad_step: x0 is required exactly when momentum != 0");
@@ -368,7 +377,8 @@ int madgrad_step(float* p, const float* g, float* nu, float* s, const float* x0,
   return 0;
 }
 
-int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t stream) {
+extern "C" int dprb_cast_f32_bf16(const float* src, void* dst, int64_t n, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0,
                "cast_f32_bf16: buffers must be 16/8-byte aligned");
   if (n == 0) return 0;
@@ -378,7 +388,8 @@ int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t stream)
   return 0;
 }
 
-int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t stream) {
+extern "C" int dprb_cast_bf16_f32(const void* src, float* dst, int64_t n, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(dst) & 15) == 0 && (reinterpret_cast<uintptr_t>(src) & 7) == 0,
                "cast_bf16_f32: buffers must be 8/16-byte aligned");
   if (n == 0) return 0;
@@ -387,5 +398,3 @@ int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t stream)
   DPRB_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace dprb

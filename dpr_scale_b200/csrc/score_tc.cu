@@ -426,14 +426,19 @@ int grid_for(long long n4, int sms) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-long long score_tc_workspace_bytes(int Q, int C, int d, int nq, int nc) {
+using namespace dprb;
+
+extern "C" int64_t dprb_score_tc_workspace_bytes(int Q, int C, int d, int nq, int nc) {
   return plan(nullptr, Q, C, d, nq < 0 ? Q : nq, nc < 0 ? C : nc).bytes;
 }
 
-int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
-                 const int64_t* labels, float inv_t, float* lse, float* loss_sum, float* logits, int Q, int C, int d,
-                 int nq, int nc, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+extern "C" int dprb_score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const uint8_t* pair_mask,
+                                 const int64_t* labels, float inv_t, float* lse, float* loss_sum, float* logits, int Q,
+                                 int C, int d, int nq, int nc, void* workspace, int64_t workspace_bytes,
+                                 dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(Q >= 0 && C > 0 && d > 0, "score_tc_fwd: bad shape Q=%d C=%d d=%d", Q, C, d);
   DPRB_REQUIRE(d % 8 == 0, "score_tc_fwd: d=%d must be a multiple of 8 (16-byte rows for TMA)", d);
   if (Q == 0) return 0;
@@ -441,7 +446,8 @@ int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(c)) & 15) == 0, "score_tc_fwd: q / c must be 16-byte aligned");
   ScoreWs w = plan(workspace, Q, C, d, nq < 0 ? Q : nq, nc < 0 ? C : nc);
   DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= w.bytes && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
-               "score_tc_fwd: workspace missing, misaligned or too small (%lld < %lld)", workspace_bytes, w.bytes);
+               "score_tc_fwd: workspace missing, misaligned or too small (%lld < %lld)", (long long)workspace_bytes,
+               w.bytes);
   if (int rc = set_attr()) return rc;
   DPRB_NUM_SMS(sms);
   const long long nqd = (long long)Q * d, ncd = (long long)C * d;
@@ -466,9 +472,11 @@ int score_tc_fwd(const float* q, const float* c, const uint8_t* col_mask, const 
   return 0;
 }
 
-int score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const int64_t* labels, const float* lse,
-                 float grad_scale, float inv_t, float* dq, float* dc, int Q, int C, int d, int q0, int nq, int c0, int nc,
-                 void* workspace, long long workspace_bytes, cudaStream_t stream) {
+extern "C" int dprb_score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const int64_t* labels,
+                                 const float* lse, float grad_scale, float inv_t, float* dq, float* dc, int Q, int C,
+                                 int d, int q0, int nq, int c0, int nc, void* workspace, int64_t workspace_bytes,
+                                 dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(Q > 0 && C > 0 && d > 0, "score_tc_bwd: bad shape Q=%d C=%d d=%d", Q, C, d);
   DPRB_REQUIRE(d % 8 == 0, "score_tc_bwd: d=%d must be a multiple of 8 (16-byte rows for TMA)", d);
   DPRB_REQUIRE(q0 >= 0 && nq >= 0 && q0 + nq <= Q && c0 >= 0 && nc >= 0 && c0 + nc <= C,
@@ -503,7 +511,7 @@ int score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const int64_
     const bf16* A[3] = {w.wr_hi, w.wr_hi, w.wr_lo};
     const bf16* B[3] = {c_h, c_m, c_h};
     for (int i = 0; i < 3; ++i)
-      if (int rc = gemm_bf16(A[i], B[i], dq, nq, d, C, w.ld_wr, d, d, 0, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0,
+      if (int rc = dprb_gemm_bf16(A[i], B[i], dq, nq, d, C, w.ld_wr, d, d, 0, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0,
                              nullptr, scale, 0, nullptr, 0.f, 0, stream)) return rc;
   }
   if (want_dc) {
@@ -512,10 +520,8 @@ int score_tc_bwd(const uint8_t* col_mask, const uint8_t* pair_mask, const int64_
     const bf16* A[3] = {w.wc_hi, w.wc_hi, w.wc_lo};
     const bf16* B[3] = {q_h, q_m, q_h};
     for (int i = 0; i < 3; ++i)
-      if (int rc = gemm_bf16(A[i], B[i], dc, nc, d, Q, w.ld_wc, d, d, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0,
+      if (int rc = dprb_gemm_bf16(A[i], B[i], dc, nc, d, Q, w.ld_wc, d, d, 1, 1, DPRB_EPI_F32_ATOMIC_ADD, nullptr, nullptr, 0,
                              nullptr, scale, 0, nullptr, 0.f, 0, stream)) return rc;
   }
   return 0;
 }
-
-}  // namespace dprb

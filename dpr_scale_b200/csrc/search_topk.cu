@@ -479,29 +479,35 @@ int kpad_for(int k) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-long long search_workspace_bytes(long long Q, int k) {
+using namespace dprb;
+
+extern "C" int64_t dprb_search_workspace_bytes(int64_t Q, int k) {
   const int sms = num_sms();
   return sms > 0 ? ws_layout(nullptr, Q, k, sms).total : -1;
 }
 
-int search_topk(const void* queries, const void* corpus, int dtype, long long Q, long long N, int d, int k,
-                long long index_offset, float* out_scores, long long* out_index, void* workspace,
-                long long workspace_bytes, cudaStream_t stream) {
-  DPRB_REQUIRE(Q > 0 && N > 0 && d > 0, "search: empty problem Q=%lld N=%lld d=%d", Q, N, d);
+extern "C" int dprb_search_topk(const void* queries, const void* corpus, int dtype, int64_t Q, int64_t N, int d, int k,
+                                int64_t index_offset, float* out_scores, int64_t* out_index_, void* workspace,
+                                int64_t workspace_bytes, dprb_stream_t stream_) {
+  long long* out_index = reinterpret_cast<long long*>(out_index_);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DPRB_REQUIRE(Q > 0 && N > 0 && d > 0, "search: empty problem Q=%lld N=%lld d=%d", (long long)Q, (long long)N, d);
   const int rank_f16 = (dtype & DPRB_SEARCH_RANK_FP16) != 0;
   dtype &= 0xFF;
   DPRB_REQUIRE(dtype == 0 || dtype == 1, "search: dtype must be 0 (fp16) or 1 (bf16), got %d", dtype);
   DPRB_REQUIRE(k >= 1 && k <= 1024, "search: k=%d outside [1, 1024]", k);
-  DPRB_REQUIRE(N >= k, "search: k=%d exceeds the %lld corpus rows (torch.topk raises here too)", k, N);
-  DPRB_REQUIRE(N < 0x7FFFFF00ll, "search: %lld corpus rows exceed the 31-bit TMA row coordinate; split into shards", N);
+  DPRB_REQUIRE(N >= k, "search: k=%d exceeds the %lld corpus rows (torch.topk raises here too)", k, (long long)N);
+  DPRB_REQUIRE(N < 0x7FFFFF00ll, "search: %lld corpus rows exceed the 31-bit TMA row coordinate; split into shards",
+               (long long)N);
   DPRB_REQUIRE(d % 8 == 0, "search: d=%d must be a multiple of 8 (16-byte rows for TMA)", d);
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(queries) & 15) == 0 && (reinterpret_cast<uintptr_t>(corpus) & 15) == 0,
                "search: operands must be 16-byte aligned");
   DPRB_NUM_SMS(sms);
   const WsLayout w = ws_layout(workspace, Q, k, sms);
   DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= w.total,
-               "search: workspace %lld B < required %lld B", workspace_bytes, w.total);
+               "search: workspace %lld B < required %lld B", (long long)workspace_bytes, w.total);
 
   static bool attr_set = false;
   if (!attr_set) {
@@ -553,18 +559,23 @@ int search_topk(const void* queries, const void* corpus, int dtype, long long Q,
   return 0;
 }
 
-long long topk_merge_workspace_bytes(long long Q, int total) {
+extern "C" int64_t dprb_topk_merge_workspace_bytes(int64_t Q, int total) {
   Carve c(nullptr);
   c.take(Q * total * (long long)sizeof(u64));
   return c.off;
 }
 
-int topk_merge(const float* scores, const long long* index, long long Q, int total, int k, float* out_scores,
-               long long* out_index, void* workspace, long long workspace_bytes, cudaStream_t stream) {
-  DPRB_REQUIRE(Q > 0 && total > 0, "topk_merge: empty problem Q=%lld total=%d", Q, total);
+extern "C" int dprb_topk_merge(const float* scores, const int64_t* index_, int64_t Q, int total, int k,
+                               float* out_scores, int64_t* out_index_, void* workspace, int64_t workspace_bytes,
+                               dprb_stream_t stream_) {
+  const long long* index = reinterpret_cast<const long long*>(index_);
+  long long* out_index = reinterpret_cast<long long*>(out_index_);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DPRB_REQUIRE(Q > 0 && total > 0, "topk_merge: empty problem Q=%lld total=%d", (long long)Q, total);
   DPRB_REQUIRE(k >= 1 && k <= 1024 && k <= total, "topk_merge: k=%d outside [1, min(1024, %d)]", k, total);
-  DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= topk_merge_workspace_bytes(Q, total),
-               "topk_merge: workspace %lld B < required %lld B", workspace_bytes, topk_merge_workspace_bytes(Q, total));
+  DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= dprb_topk_merge_workspace_bytes(Q, total),
+               "topk_merge: workspace %lld B < required %lld B", (long long)workspace_bytes,
+               (long long)dprb_topk_merge_workspace_bytes(Q, total));
   u64* keys = static_cast<u64*>(workspace);
   const long long n = Q * total;
   pack_keys_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(scores, keys, n, total);
@@ -578,5 +589,3 @@ int topk_merge(const float* scores, const long long* index, long long Q, int tot
   sl.gather = index; sl.gather_stride = total;
   return launch_select(sl, Q, stream);
 }
-
-}  // namespace dprb

@@ -204,9 +204,13 @@ seqcls_group_ce_final_kernel(const float* __restrict__ dw_part, const float* __r
 }
 
 }  // namespace
+}  // namespace dprb
 
-int seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits, float* score, int N,
-                    int H, int L, cudaStream_t stream) {
+using namespace dprb;
+
+extern "C" int dprb_seqcls_head_fwd(const float* pre, const float* weight, const float* bias, float* logits,
+                                    float* score, int N, int H, int L, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(N >= 0, "seqcls_head: N = %d must be >= 0", N);
   DPRB_REQUIRE(H > 0 && H % 8 == 0 && H <= 1024, "seqcls_head: hidden size %d must be a multiple of 8 and <= 1024", H);
   DPRB_REQUIRE(L >= 1 && L <= DPRB_SEQCLS_MAX_LABELS, "seqcls_head: %d labels (supported: 1 .. %d)", L,
@@ -221,13 +225,16 @@ int seqcls_head_fwd(const float* pre, const float* weight, const float* bias, fl
   return 0;
 }
 
-long long seqcls_group_ce_workspace_bytes(int B, int H) {
+extern "C" int64_t dprb_seqcls_group_ce_workspace_bytes(int B, int H) {
   return B > 0 && H > 0 ? ((long long)B * H + 2LL * B) * (long long)sizeof(float) : 0;
 }
 
-int seqcls_group_ce(const float* pre, const float* weight, const float* bias, const long long* labels, int B, int G,
-                    int H, float dropout_p, unsigned long long dropout_seed, float* loss, float* logits, void* dpre,
-                    float* dweight, float* dbias, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+extern "C" int dprb_seqcls_group_ce(const float* pre, const float* weight, const float* bias, const int64_t* labels_,
+                                    int B, int G, int H, float dropout_p, uint64_t dropout_seed, float* loss,
+                                    float* logits, void* dpre, float* dweight, float* dbias, void* workspace,
+                                    int64_t workspace_bytes, dprb_stream_t stream_) {
+  const long long* labels = reinterpret_cast<const long long*>(labels_);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(B >= 1, "seqcls_group_ce: %d groups (at least 1)", B);
   DPRB_REQUIRE(G >= 2 && G <= DPRB_SEQCLS_GROUP_MAX, "seqcls_group_ce: group size %d (supported: 2 .. %d)", G,
                DPRB_SEQCLS_GROUP_MAX);
@@ -241,9 +248,9 @@ int seqcls_group_ce(const float* pre, const float* weight, const float* bias, co
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(weight) |
                  reinterpret_cast<uintptr_t>(dpre) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
                "seqcls_group_ce: pre, weight, dpre and workspace must be 16-byte aligned");
-  const long long need = seqcls_group_ce_workspace_bytes(B, H);
+  const long long need = dprb_seqcls_group_ce_workspace_bytes(B, H);
   DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= need, "seqcls_group_ce: workspace of %lld bytes, %lld needed",
-               workspace_bytes, need);
+               (long long)workspace_bytes, need);
   float* dw_part = reinterpret_cast<float*>(workspace);
   float* db_part = dw_part + (size_t)B * H;
   float* loss_part = db_part + B;
@@ -257,5 +264,3 @@ int seqcls_group_ce(const float* pre, const float* weight, const float* bias, co
   DPRB_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace dprb

@@ -81,24 +81,32 @@ sparse_search_kernel(const SparseParams p) {
 }
 
 }  // namespace
+}  // namespace dprb
 
-int sparse_search_block_queries(long long N) { return fixed_acc_block_queries(N); }
+using namespace dprb;
 
-long long sparse_search_workspace_bytes(long long N, int Qb) { return fixed_acc_workspace_bytes(N, Qb); }
+extern "C" int dprb_sparse_search_block_queries(int64_t N) { return fixed_acc_block_queries(N); }
 
-int sparse_search(const int32_t* row, const void* weight, const long long* term_ptr, long long nnz, int V,
-                  const long long* row_ids, long long N, const int32_t* q_term, const float* q_weight,
-                  const int32_t* q_seq, const int32_t* item_end, int Eq, int items, int Qb, int k, float* out_scores,
-                  long long* out_ids, void* workspace, long long workspace_bytes, cudaStream_t stream) {
-  DPRB_REQUIRE(N >= 1 && N < (1LL << 31), "sparse_search: N=%lld passages outside [1, 2^31)", N);
+extern "C" int64_t dprb_sparse_search_workspace_bytes(int64_t N, int Qb) { return fixed_acc_workspace_bytes(N, Qb); }
+
+extern "C" int dprb_sparse_search(const int32_t* row, const void* weight, const int64_t* term_ptr_, int64_t nnz, int V,
+                                  const int64_t* row_ids_, int64_t N, const int32_t* q_term, const float* q_weight,
+                                  const int32_t* q_seq, const int32_t* item_end, int Eq, int items, int Qb, int k,
+                                  float* out_scores, int64_t* out_ids_, void* workspace, int64_t workspace_bytes,
+                                  dprb_stream_t stream_) {
+  const long long* term_ptr = reinterpret_cast<const long long*>(term_ptr_);
+  const long long* row_ids = reinterpret_cast<const long long*>(row_ids_);
+  long long* out_ids = reinterpret_cast<long long*>(out_ids_);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DPRB_REQUIRE(N >= 1 && N < (1LL << 31), "sparse_search: N=%lld passages outside [1, 2^31)", (long long)N);
   DPRB_REQUIRE(V >= 1, "sparse_search: V=%d terms, at least 1 needed", V);
-  DPRB_REQUIRE(nnz >= 0 && nnz < (1LL << 40), "sparse_search: nnz=%lld postings outside [0, 2^40)", nnz);
+  DPRB_REQUIRE(nnz >= 0 && nnz < (1LL << 40), "sparse_search: nnz=%lld postings outside [0, 2^40)", (long long)nnz);
   DPRB_REQUIRE(Eq >= 0 && items >= 0 && (Eq > 0 || items == 0),
                "sparse_search: Eq=%d query entries, %d work items", Eq, items);
-  DPRB_REQUIRE(k >= 1 && k <= 1024 && k <= N, "sparse_search: k=%d outside [1, min(1024, N=%lld)]", k, N);
-  DPRB_REQUIRE(Qb >= 1 && Qb <= sparse_search_block_queries(N),
+  DPRB_REQUIRE(k >= 1 && k <= 1024 && k <= N, "sparse_search: k=%d outside [1, min(1024, N=%lld)]", k, (long long)N);
+  DPRB_REQUIRE(Qb >= 1 && Qb <= dprb_sparse_search_block_queries(N),
                "sparse_search: Qb=%d queries per block outside [1, %d] (dprb_sparse_search_block_queries)", Qb,
-               sparse_search_block_queries(N));
+               dprb_sparse_search_block_queries(N));
   DPRB_REQUIRE(term_ptr != nullptr, "sparse_search: NULL term_ptr");
   DPRB_REQUIRE(nnz == 0 || (row != nullptr && weight != nullptr), "sparse_search: NULL posting operand");
   DPRB_REQUIRE(Eq == 0 || (q_term != nullptr && q_weight != nullptr && q_seq != nullptr && item_end != nullptr),
@@ -106,9 +114,9 @@ int sparse_search(const int32_t* row, const void* weight, const long long* term_
   DPRB_REQUIRE(out_scores != nullptr && out_ids != nullptr, "sparse_search: NULL output");
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(row) | reinterpret_cast<uintptr_t>(weight)) & 15) == 0,
                "sparse_search: posting arrays must be 16-byte aligned");
-  const long long need = sparse_search_workspace_bytes(N, Qb);
+  const long long need = dprb_sparse_search_workspace_bytes(N, Qb);
   DPRB_REQUIRE(workspace != nullptr && workspace_bytes >= need && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
-               "sparse_search: workspace of %lld bytes (256-byte aligned), %lld needed", workspace_bytes, need);
+               "sparse_search: workspace of %lld bytes (256-byte aligned), %lld needed", (long long)workspace_bytes, need);
   DPRB_NUM_SMS(sms);
 
   FixedAcc fa;
@@ -131,5 +139,3 @@ int sparse_search(const int32_t* row, const void* weight, const long long* term_
   }
   return fixed_acc_select(fa.acc, N, Qb, k, row_ids, out_scores, out_ids, stream);
 }
-
-}  // namespace dprb

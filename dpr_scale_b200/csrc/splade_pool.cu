@@ -246,15 +246,22 @@ int make_tmap_rows(CUtensorMap* out, const void* base, long long rows, int K, lo
 }
 
 }  // namespace
+}  // namespace dprb
 
-int splade_pool_fwd(const void* x, long long ldx, const void* W, long long ldw, const float* bias, const int32_t* off,
-                    long long T, int N, int V, int K, float* out, long long ldo, cudaStream_t stream) {
+using namespace dprb;
+
+extern "C" int dprb_splade_pool_fwd(const void* x, int64_t ldx, const void* W, int64_t ldw, const float* bias,
+                                    const int32_t* off, int64_t T, int N, int V, int K, float* out, int64_t ldo,
+                                    dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(K % 8 == 0 && K >= 8 && K <= MAX_K, "splade_pool_fwd: K=%d unsupported (multiple of 8, 8 .. 1024)", K);
   DPRB_REQUIRE(ldx >= K && ldx % 8 == 0 && ldw >= K && ldw % 8 == 0,
-               "splade_pool_fwd: ldx=%lld ldw=%lld must be multiples of 8 and at least K=%d", ldx, ldw, K);
+               "splade_pool_fwd: ldx=%lld ldw=%lld must be multiples of 8 and at least K=%d", (long long)ldx,
+               (long long)ldw, K);
   DPRB_REQUIRE(V >= 1 && N >= 1, "splade_pool_fwd: V=%d N=%d (both at least 1)", V, N);
-  DPRB_REQUIRE(ldo >= V, "splade_pool_fwd: ldo=%lld < V=%d", ldo, V);
-  DPRB_REQUIRE(T >= 0 && T < 0x7FFFFF00LL, "splade_pool_fwd: T=%lld rows outside [0, 2^31) (32-bit row indices)", T);
+  DPRB_REQUIRE(ldo >= V, "splade_pool_fwd: ldo=%lld < V=%d", (long long)ldo, V);
+  DPRB_REQUIRE(T >= 0 && T < 0x7FFFFF00LL, "splade_pool_fwd: T=%lld rows outside [0, 2^31) (32-bit row indices)",
+               (long long)T);
   DPRB_REQUIRE(off != nullptr && out != nullptr && (T == 0 || (x != nullptr && W != nullptr)),
                "splade_pool_fwd: NULL operand");
   DPRB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
@@ -286,5 +293,3 @@ int splade_pool_fwd(const void* x, long long ldx, const void* W, long long ldw, 
   DPRB_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace dprb

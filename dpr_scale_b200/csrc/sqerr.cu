@@ -87,20 +87,27 @@ sqerr_final_kernel(const double* __restrict__ partial, int n, float* __restrict_
 }
 
 }  // namespace
+}  // namespace dprb
 
-long long sqerr_workspace_bytes(int rows) {
+using namespace dprb;
+
+// The workspace holds one double per block, and the grid depends on rows alone: d does not size it.
+extern "C" int64_t dprb_sqerr_workspace_bytes(int rows, int d) {
+  (void)d;
   return rows > 0 ? (long long)sqerr_blocks(rows) * (long long)sizeof(double) : 0;
 }
 
-int sqerr_fwd(const float* x, long long ldx, const float* t, long long ldt, int rows, int d, float* loss_sum, float* dx,
-              long long lddx, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+extern "C" int dprb_sqerr_fwd(const float* x, int64_t ldx, const float* t, int64_t ldt, int rows, int d, float* loss_sum,
+                              float* dx, int64_t lddx, void* workspace, int64_t workspace_bytes, dprb_stream_t stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DPRB_REQUIRE(rows >= 0 && d >= 1, "sqerr_fwd: rows=%d d=%d (rows >= 0, d >= 1)", rows, d);
   DPRB_REQUIRE(ldx >= d && ldt >= d && (dx == nullptr || lddx >= d),
-               "sqerr_fwd: ldx=%lld ldt=%lld lddx=%lld must be at least d=%d", ldx, ldt, lddx, d);
+               "sqerr_fwd: ldx=%lld ldt=%lld lddx=%lld must be at least d=%d", (long long)ldx, (long long)ldt,
+               (long long)lddx, d);
   DPRB_REQUIRE(loss_sum != nullptr && (rows == 0 || (x != nullptr && t != nullptr)), "sqerr_fwd: NULL operand");
-  const long long need = sqerr_workspace_bytes(rows);
+  const long long need = dprb_sqerr_workspace_bytes(rows, d);
   DPRB_REQUIRE(workspace_bytes >= need && (need == 0 || workspace != nullptr),
-               "sqerr_fwd: workspace of %lld bytes, %lld needed", workspace_bytes, need);
+               "sqerr_fwd: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, need);
   DPRB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "sqerr_fwd: workspace must be 8-byte aligned");
   double* partial = reinterpret_cast<double*>(workspace);
   const int blocks = rows > 0 ? sqerr_blocks(rows) : 0;
@@ -118,5 +125,3 @@ int sqerr_fwd(const float* x, long long ldx, const float* t, long long ldt, int 
   DPRB_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace dprb

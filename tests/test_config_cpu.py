@@ -29,10 +29,38 @@ def test_instantiate_task_by_target_without_recursion():
     assert task.shared_model is False and task.in_batch_negatives is True
 
 
-def test_library_exports_every_declared_symbol():
-    header = open(os.path.join(ROOT, "include", "dprb.h")).read()
-    declared = set(re.findall(r"\b(dprb_[a-z0-9_]+)\s*\(", header))
+def test_signatures_match_every_header_prototype():
+    """_lib.SIGNATURES binds exactly the entry points include/dprb.h declares, each with the header's return type and
+    argument list: a pointer or dprb_stream_t as c_void_p or a ctypes POINTER, int / int64_t / uint64_t / float as
+    their ctypes twins.  The built library exports every one of them."""
+    scalar = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "float": ctypes.c_float,
+              "const char*": ctypes.c_char_p}
+    header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "dprb.h")).read(), flags=re.S)
+    protos = re.findall(r"^(\w[\w ]*?\**)\s*\b(dprb_\w+)\(([^)]*)\);", header, flags=re.M)
+    declared = {name for _, name, _ in protos}
+    assert len(declared) == len(protos)
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
+
+    def is_pointer(t):
+        return t is ctypes.c_void_p or (isinstance(t, type) and issubclass(t, ctypes._Pointer))
+
+    bad = []
+    for ret, name, params in protos:
+        restype, argtypes = _lib.SIGNATURES[name]
+        if restype is not scalar.get(ret.strip()):
+            bad.append(f"{name}: returns {ret.strip()}, bound as {restype.__name__}")
+        params = [] if params.strip() == "void" else [" ".join(p.split()) for p in params.split(",")]
+        if len(params) != len(argtypes):
+            bad.append(f"{name}: {len(params)} arguments declared, {len(argtypes)} bound")
+            continue
+        for i, (p, t) in enumerate(zip(params, argtypes)):
+            if "*" in p or p.startswith("dprb_stream_t "):
+                ok = is_pointer(t)
+            else:
+                ok = t is scalar.get(p.rsplit(" ", 1)[0])
+            if not ok:
+                bad.append(f"{name}: argument {i} `{p}` bound as {t.__name__}")
+    assert not bad, "\n".join(bad)
     lib = ctypes.CDLL(_lib.LIB_PATH)
     for name in declared:
         assert hasattr(lib, name), name

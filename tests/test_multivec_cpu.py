@@ -8,8 +8,7 @@
     its rerank scores for both pools;
   * refusals raise ValueError without a GPU: a grad-enabled forward, topk > 8, P or Pc out of range, an unsupported
     model type;
-  * the YAML groups compose, and dprb_maxsim_expert_fwd is declared in include/dprb.h, bound in _lib.SIGNATURES and
-    exported by the built library.
+  * the YAML groups compose.
 """
 import json
 import os
@@ -23,7 +22,6 @@ from tests.util import GOLDEN
 
 RAW = np.load(os.path.join(GOLDEN, "multivec_small.npz"))
 G = {k: torch.from_numpy(RAW[k]) for k in RAW.files if RAW[k].dtype.kind != "U"}
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NAMES = list(multivec_cases.TINY)
 
 
@@ -177,15 +175,3 @@ def test_config_composes(model):
     for k, v in dims.items():
         assert cfg.task.model[k] == v
     assert cfg.task.model.dropout == 0.1 and cfg.task.add_cls is True and cfg.task.query_topk == 2
-
-
-def test_entry_point_declared_bound_and_exported():
-    from dpr_scale_b200 import _lib
-    header = open(os.path.join(ROOT, "include", "dprb.h")).read()
-    assert "int dprb_maxsim_expert_fwd(" in header
-    assert "dprb_maxsim_expert_fwd" in _lib.SIGNATURES
-    assert len(_lib.SIGNATURES["dprb_maxsim_expert_fwd"][1]) == 20
-    if os.path.exists(_lib.LIB_PATH):
-        import subprocess
-        syms = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True).stdout
-        assert " dprb_maxsim_expert_fwd" in syms

@@ -5,8 +5,7 @@
     reference wrote, exactly once rounded to fp32, keys and entry order included;
   * the task and datamodule configs compose, and the query collate equals the reference's batches;
   * refusals raise ValueError without a GPU: a ColBERT encoder, a query batch without topic ids, a grad-enabled step,
-    a non-integer corpus id, shapes outside the kernel's limits;
-  * dprb_expert_group is declared in include/dprb.h, bound in _lib.SIGNATURES and exported by the built library.
+    a non-integer corpus id, shapes outside the kernel's limits.
 """
 import json
 import os
@@ -19,7 +18,6 @@ from tests import colbert_cases, multivec_cases, multivec_index_cases as cases, 
 from tests.util import GOLDEN
 
 G = np.load(os.path.join(GOLDEN, "multivec_index_small.npz"))
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KEYS = ("expert_repr", "expert_ids", "expert_weights", "attention_mask")
 
 
@@ -158,15 +156,3 @@ def test_expert_group_check_limits():
                  (2, 16, 1, 32, 0), (2, 16, 1, 32, 1 << 24), (1 << 20, 512, 8, 32, 100)):
         with pytest.raises(ValueError):
             ops.expert_group_check(*args)
-
-
-def test_entry_point_declared_bound_and_exported():
-    from dpr_scale_b200 import _lib
-    header = open(os.path.join(ROOT, "include", "dprb.h")).read()
-    for name, nargs in (("dprb_expert_group", 22), ("dprb_expert_group_workspace_bytes", 3)):
-        assert f" {name}(" in header
-        assert len(_lib.SIGNATURES[name][1]) == nargs
-    if os.path.exists(_lib.LIB_PATH):
-        import subprocess
-        syms = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True).stdout
-        assert " dprb_expert_group" in syms and " dprb_expert_group_workspace_bytes" in syms

@@ -8,8 +8,7 @@
   * the task config composes;
   * refusals raise ValueError before any GPU work: the options whose behaviour lives in the reference's missing index
     module, shapes outside the kernel limits, an id missing from the passage table, a CLS row count other than N,
-    add_cls without CLS files, a payload width other than the encoder's, an add_context_id index;
-  * dprb_expert_search is declared in include/dprb.h, bound in _lib.SIGNATURES and exported by the built library.
+    add_cls without CLS files, a payload width other than the encoder's, an add_context_id index.
 """
 import json
 import os
@@ -191,20 +190,6 @@ def test_index_load_refusals(tmp_path):
         pickle.dump((torch.tensor([1]), torch.ones(1), torch.tensor([7.0])), f, protocol=4)
     with pytest.raises(ValueError, match="add_context_id"):
         ExpertIndex.load(str(tmp_path / "ctx"), ids, device="cpu")
-
-
-def test_entry_point_declared_bound_and_exported():
-    from dpr_scale_b200 import _lib
-    header = open(os.path.join(ROOT, "include", "dprb.h")).read()
-    for name, nargs in (("dprb_expert_search", 27), ("dprb_expert_search_workspace_bytes", 2),
-                        ("dprb_expert_search_block_queries", 1)):
-        assert f" {name}(" in header
-        assert len(_lib.SIGNATURES[name][1]) == nargs
-    if os.path.exists(_lib.LIB_PATH):
-        import subprocess
-        syms = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True).stdout
-        for name in ("dprb_expert_search", "dprb_expert_search_workspace_bytes", "dprb_expert_search_block_queries"):
-            assert f" {name}\n" in syms
 
 
 # ---- against the unmodified reference (tests/golden/make_golden_multivec_retrieval.py)

@@ -6,8 +6,7 @@
   * the float64 oracle (oracle/splade.py) against the reference's SPLADE reps and both encoders' rerank pickles;
   * refusals raise ValueError without a GPU (a grad-enabled forward, sequence lengths, model types, widths) and
     ops.splade_pool_check mirrors dprb_splade_pool_fwd's limits;
-  * the YAML groups compose, and dprb_splade_pool_fwd is declared in include/dprb.h, bound in _lib.SIGNATURES and
-    exported by the built library.
+  * the YAML groups compose.
 """
 import json
 import os
@@ -21,7 +20,6 @@ from tests.util import GOLDEN
 
 RAW = np.load(os.path.join(GOLDEN, "splade_small.npz"))
 G = {k: torch.from_numpy(RAW[k]) for k in RAW.files if RAW[k].dtype.kind != "U"}
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NAMES = list(splade_cases.TINY)
 
 
@@ -171,15 +169,3 @@ def test_config_composes(model):
     assert cfg.datamodule._target_ == "dpr_scale_b200.datamodule.citadel.DenseRetrieverRerankDataModule"
     assert cfg.task.model.dropout == 0.1 and cfg.task.shared_model is False and cfg.task.in_batch_eval is False
     assert cfg.task.checkpoint_path == "/c" and cfg.task.output_dir == "/o"
-
-
-def test_entry_point_declared_bound_and_exported():
-    from dpr_scale_b200 import _lib
-    header = open(os.path.join(ROOT, "include", "dprb.h")).read()
-    assert "int dprb_splade_pool_fwd(" in header
-    assert "dprb_splade_pool_fwd" in _lib.SIGNATURES
-    assert len(_lib.SIGNATURES["dprb_splade_pool_fwd"][1]) == 13
-    if os.path.exists(_lib.LIB_PATH):
-        import subprocess
-        syms = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True).stdout
-        assert " dprb_splade_pool_fwd" in syms

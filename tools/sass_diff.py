@@ -3,8 +3,9 @@
     python tools/sass_diff.py OLD/libdprb.so NEW/libdprb.so [--expect-changed SUBSTR ...]
 
 Runs `cuobjdump -sass` on both libraries, splits the listings at `Function :` and compares each kernel's
-instructions.  Anonymous-namespace hashes (`_GLOBAL__N__<hex>_`) change whenever a file's text changes, so they are
-replaced by a fixed token first, and runs of whitespace are collapsed.  A refactor that should not touch device code passes when every kernel is identical;
+instructions.  nvcc names a file's anonymous namespace `_GLOBAL__N__<hash>_<len>_<file>_cu_<hash2>`, and both hashes
+change whenever the file's text changes, so the whole token is replaced by a fixed one first, and runs of whitespace
+are collapsed.  A refactor that should not touch device code passes when every kernel is identical;
 kernels that are meant to change are named with --expect-changed (a substring of the mangled name).  Exit code 1 when
 a kernel is missing on one side or differs without being expected to.  No GPU is needed.
 """
@@ -14,7 +15,7 @@ import re
 import subprocess
 import sys
 
-_ANON = re.compile(r"_GLOBAL__N__[0-9a-f]+_")
+_ANON = re.compile(r"_GLOBAL__N__[0-9a-f]+_([0-9]+_\w+?_cu_)?[0-9a-f]{8}")
 
 
 def kernels(lib):
